@@ -7,14 +7,17 @@
 // texture_view.cpp:157,215,224.
 //
 // Pipeline (all faces of the context's face range, all views):
-//   cull<count>  : back-face / frustum / 75 degree / 3-vertex validity  -> candidates per face
+//   cull<count>  : back-face / frustum / 75 degree / 3-vertex validity, thread per face -> candidates per
+//                  face + one bit per surviving view (pass_bits[face][ceil(K/32)])
 //   scan         : candidate offsets (CSR by face)
-//   cull<fill>   : candidate (face,view) list + the set of (vertex,view) rays that are needed
+//   cull<fill>   : candidate (face,view) list + the set of (vertex,view) rays that are needed; warp per face,
+//                  lane l of pass word w owns view 32w+l, so the list is written in contiguous runs
 //   rays         : ONE visibility ray per needed (vertex,view) -- the reference traces the same ray
 //                  once per incident face (calculate_data_costs.cpp:197-213); the result depends only
 //                  on (vertex, view), so it is shared (about 6x fewer rays, identical answers)
 //   quality      : occlusion lookup + footprint integral (GMI) per candidate, global max
-//   compact      : drop quality==0, CSR by face with ascending views (:222, :272)
+//   count_survivors -> scan -> compact : drop quality==0, CSR by face with ascending views (:222, :272);
+//                  the compaction runs warp per face, 32-candidate chunks, prefix popcount of the survivor mask
 //   histogram -> percentile -> normalise (:277-302, histogram.cpp:22-63)
 #include <cub/cub.cuh>
 
@@ -131,6 +134,86 @@ __device__ __forceinline__ bool cull_pair(const ViewDev &V, const FaceGeom &g, f
     return valid_pixel(V, p3);
 }
 
+// The candidate kernels run one WARP per face where they touch the candidate list (grid-stride over the faces), so that
+// the ~44 candidates of a face are read and written by neighbouring lanes: contiguous runs instead of one thread per face
+// striding 44 elements.  A lane gets its slot from a 32-bit mask of the face's current 32 candidates that every lane
+// forms itself from the same (broadcast) loads, so the kernels need no warp collective and each lane's work depends on
+// nothing but memory: the host emulation (tests/cpp/cuda_emul.h) runs them thread after thread.
+__device__ __forceinline__ uint32_t lanemask_lt() { return (1u << (threadIdx.x & 31u)) - 1u; }
+__device__ __forceinline__ uint32_t warp_id() { return (blockIdx.x * blockDim.x + threadIdx.x) >> 5; }
+__device__ __forceinline__ uint32_t num_warps() { return (gridDim.x * blockDim.x) >> 5; }
+
+// count pass, thread per face, loop over the K views: the surviving views go to pass_bits[f - face_begin][kwords]
+// (bit j of word j/32 = view j), their number to cand_cnt[f]
+__device__ __forceinline__ void cull_count(const float *__restrict__ verts, const uint32_t *__restrict__ faces,
+                                           const float *__restrict__ normals, const ViewDev *__restrict__ views, uint32_t K,
+                                           uint32_t face_begin, uint32_t face_end, float cos_thr, uint64_t *cand_cnt,
+                                           uint32_t *pass_bits, uint32_t kwords)
+{
+    uint32_t f = face_begin + blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= face_end) return;
+    FaceGeom g;
+    uint32_t vid[3];
+    load_face(verts, faces, normals, f, g, vid);
+    const float margin = 1e-5f * fmaxf(1.0f, sqrtf(g.n[0] * g.n[0] + g.n[1] * g.n[1] + g.n[2] * g.n[2]));
+    uint32_t count = 0;
+    uint32_t bits = 0;
+    for (uint32_t j = 0; j < K; ++j) {
+        const bool pass = cull_pair(views[j], g, cos_thr, margin);
+        if (pass) bits |= 1u << (j & 31u);
+        if ((j & 31u) == 31u || j + 1 == K) { pass_bits[(size_t)(f - face_begin) * kwords + (j >> 5)] = bits; bits = 0; }
+        count += pass;
+    }
+    cand_cnt[f] = count;
+}
+
+// fill pass, warp per face: the (face, view) list in CSR order (views ascending) from the pass bits, and the set of
+// (vertex, view) rays that are needed.  Lane l of pass word w owns view 32w+l; its slot is the face's offset + the
+// candidates of the earlier words + the set bits below l.
+__device__ __forceinline__ void cull_fill(const uint32_t *__restrict__ faces, uint32_t face_begin, uint32_t face_end,
+                                          const uint64_t *__restrict__ cand_ptr, uint16_t *cand_view, uint32_t *cand_face,
+                                          uint32_t *need_bits, uint32_t vwords, const uint32_t *__restrict__ vrank,
+                                          const uint32_t *__restrict__ pass_bits, uint32_t kwords)
+{
+    const uint32_t lane = threadIdx.x & 31u, lt = lanemask_lt();
+    for (uint32_t f = face_begin + warp_id(); f < face_end; f += num_warps()) {
+        uint64_t o = cand_ptr[f];
+        // ray bitmaps are indexed by the Morton rank of the vertex so that a warp of k_rays traces 32 spatially
+        // adjacent origins towards the same camera.  Vertices of the face that share a bitmap word share one update.
+        uint32_t vw[3] = {0, 0, 0}, vb[3] = {0, 0, 0};
+        if (need_bits) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const uint32_t r = vrank[faces[3 * (size_t)f + k]];
+                vw[k] = r >> 5; vb[k] = 1u << (r & 31u);
+            }
+            if (vw[1] == vw[0]) { vb[0] |= vb[1]; vb[1] = 0; }
+            if (vw[2] == vw[0]) { vb[0] |= vb[2]; vb[2] = 0; }
+            else if (vw[2] == vw[1] && vb[1]) { vb[1] |= vb[2]; vb[2] = 0; }
+        }
+        const uint32_t *pb = pass_bits + (size_t)(f - face_begin) * kwords;
+        for (uint32_t w = 0; w < kwords; ++w) {
+            const uint32_t word = pb[w];   // the same address in every lane: one transaction
+            if ((word >> lane) & 1u) {
+                const uint32_t j = 32u * w + lane;
+                const uint64_t slot = o + __popc(word & lt);
+                cand_view[slot] = (uint16_t)j;
+                cand_face[slot] = f;
+                if (need_bits) {
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        if (!vb[k]) continue;
+                        uint32_t *p = need_bits + (size_t)j * vwords + vw[k];
+                        if ((*p & vb[k]) != vb[k]) atomicOr(p, vb[k]);
+                    }
+                }
+            }
+            o += __popc(word);
+        }
+    }
+}
+
+// count: thread per face (launch with >= face_end - face_begin threads); fill: warp per face (any grid)
 template <bool FILL>
 __global__ void __launch_bounds__(256) k_cull(const float *__restrict__ verts, const uint32_t *__restrict__ faces,
                                               const float *__restrict__ normals, const ViewDev *__restrict__ views,
@@ -140,46 +223,8 @@ __global__ void __launch_bounds__(256) k_cull(const float *__restrict__ verts, c
                                               uint32_t vwords, const uint32_t *__restrict__ vrank,
                                               uint32_t *pass_bits, uint32_t kwords)
 {
-    uint32_t f = face_begin + blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= face_end) return;
-    FaceGeom g;
-    uint32_t vid[3];
-    load_face(verts, faces, FILL ? nullptr : normals, f, g, vid);
-    const float margin = FILL ? 0.0f
-                              : 1e-5f * fmaxf(1.0f, sqrtf(g.n[0] * g.n[0] + g.n[1] * g.n[1] + g.n[2] * g.n[2]));
-    uint64_t base = FILL ? cand_ptr[f] : 0;
-    uint32_t count = 0;
-    // ray bitmaps are indexed by the Morton rank of the vertex so that a warp of k_rays traces 32
-    // spatially adjacent origins towards the same camera
-    uint32_t vr[3] = {0, 0, 0};
-    if (FILL && need_bits) { vr[0] = vrank[vid[0]]; vr[1] = vrank[vid[1]]; vr[2] = vrank[vid[2]]; }
-    uint32_t bits = 0;
-    for (uint32_t j = 0; j < K; ++j) {
-        // the count pass records which views survive; the fill pass only replays the set bits
-        if (FILL) {
-            if ((j & 31u) == 0) bits = pass_bits[(size_t)(f - face_begin) * kwords + (j >> 5)];
-            if (!((bits >> (j & 31u)) & 1u)) continue;
-        } else {
-            const bool pass = cull_pair(views[j], g, cos_thr, margin);
-            if (pass) bits |= 1u << (j & 31u);
-            if ((j & 31u) == 31u || j + 1 == K) { pass_bits[(size_t)(f - face_begin) * kwords + (j >> 5)] = bits; bits = 0; }
-            if (!pass) continue;
-        }
-        if (FILL) {
-            cand_view[base + count] = (uint16_t)j;
-            cand_face[base + count] = f;
-            if (need_bits) {
-#pragma unroll
-                for (int k = 0; k < 3; ++k) {
-                    size_t word = (size_t)j * vwords + (vr[k] >> 5);
-                    uint32_t bit = 1u << (vr[k] & 31);
-                    if (!(need_bits[word] & bit)) atomicOr(&need_bits[word], bit);
-                }
-            }
-        }
-        ++count;
-    }
-    if (!FILL) cand_cnt[f] = count;
+    if (FILL) cull_fill(faces, face_begin, face_end, cand_ptr, cand_view, cand_face, need_bits, vwords, vrank, pass_bits, kwords);
+    else cull_count(verts, faces, normals, views, K, face_begin, face_end, cos_thr, cand_cnt, pass_bits, kwords);
 }
 
 // one warp = 32 consecutive vertices of one view; lane 0 publishes the 32 occlusion bits
@@ -522,16 +567,28 @@ __global__ void k_count_survivors(const uint64_t *__restrict__ cand_ptr, const f
     cnt[f] = n;
 }
 
-__global__ void k_compact(const uint64_t *__restrict__ cand_ptr, const float *__restrict__ cand_q,
-                          const uint16_t *__restrict__ cand_view, const uint64_t *__restrict__ dc_ptr,
-                          uint32_t face_begin, uint32_t face_end, uint16_t *dc_view, float *dc_quality)
+// drop quality 0, warp per face in 32-candidate chunks: bit k of `m` = candidate c+k survives, so a kept candidate's slot
+// is the face's offset + the survivors of the earlier chunks + popc(m & lanemask_lt), and the DataCosts rows are written
+// in contiguous runs in candidate (= ascending view) order
+__global__ void __launch_bounds__(256) k_compact(const uint64_t *__restrict__ cand_ptr, const float *__restrict__ cand_q,
+                                                 const uint16_t *__restrict__ cand_view, const uint64_t *__restrict__ dc_ptr,
+                                                 uint32_t face_begin, uint32_t face_end, uint16_t *dc_view, float *dc_quality)
 {
-    uint32_t f = face_begin + blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= face_end) return;
-    uint64_t o = dc_ptr[f];
-    for (uint64_t i = cand_ptr[f]; i < cand_ptr[f + 1]; ++i) {
-        float q = cand_q[i];
-        if (q != 0.0f) { dc_view[o] = cand_view[i]; dc_quality[o] = q; ++o; }
+    const uint32_t lane = threadIdx.x & 31u, lt = lanemask_lt();
+    for (uint32_t f = face_begin + warp_id(); f < face_end; f += num_warps()) {
+        const uint64_t a = cand_ptr[f], b = cand_ptr[f + 1];
+        uint64_t o = dc_ptr[f];
+        for (uint64_t c = a; c < b; c += 32) {
+            const uint32_t n = b - c < 32 ? (uint32_t)(b - c) : 32u;
+            uint32_t m = 0;
+            for (uint32_t k = 0; k < n; ++k) m |= (uint32_t)(cand_q[c + k] != 0.0f) << k;   // broadcast loads of one chunk
+            if ((m >> lane) & 1u) {
+                const uint64_t slot = o + __popc(m & lt);
+                dc_view[slot] = cand_view[c + lane];
+                dc_quality[slot] = cand_q[c + lane];
+            }
+            o += __popc(m);
+        }
     }
 }
 
@@ -585,13 +642,21 @@ float cos75_threshold()
 
 }  // namespace
 
+// grid of the warp-per-face kernels (256 threads = 8 warps per block): one warp per face up to a full-occupancy wave,
+// beyond that the warps loop over the faces
+static unsigned face_warp_blocks(const b2tex_ctx *c, uint64_t faces)
+{
+    const uint64_t want = (faces + 7) / 8;
+    const uint64_t wave = (uint64_t)std::max(1, c->num_sms) * 8;
+    return (unsigned)std::max<uint64_t>(1, std::min(want, wave));
+}
+
 // qualities of all candidates are known: photometric outlier removal (optional), drop quality 0, compact to the
 // DataCosts layout, maximum (calculate_data_costs.cpp:222,265-281)
 static int finish_candidates(b2tex_ctx *c, const b2tex_settings *st, uint64_t num_cand, b2tex_dc_info *info)
 {
     cudaStream_t s = c->stream;
     const uint32_t F = c->F, fb = c->face_begin, fe = c->face_end, nf = fe - fb;
-    const uint32_t blocks = (nf + 255) / 256;
     const bool outlier = st->outlier_removal != 0;
     DevBuf<uint64_t> &cnt = c->s_cnt64;
     unsigned long long *ray_count = reinterpret_cast<unsigned long long *>(c->scalars.p + 2);
@@ -626,7 +691,7 @@ static int finish_candidates(b2tex_ctx *c, const b2tex_settings *st, uint64_t nu
     B2_TRY(c->dc_cost.alloc(nnz));
     if (nf) {
         ScopedTimer tm(c, "k_compact", 6.0 * (double)num_cand + 6.0 * (double)nnz + 16.0 * nf);
-        B2_LAUNCH k_compact<<<blocks, 256, 0, s>>>(c->cand_ptr.p, c->cand_q.p, c->cand_view.p, c->dc_ptr.p, fb, fe,
+        B2_LAUNCH k_compact<<<face_warp_blocks(c, nf), 256, 0, s>>>(c->cand_ptr.p, c->cand_q.p, c->cand_view.p, c->dc_ptr.p, fb, fe,
                                          c->dc_view.p, c->dc_quality.p);
     }
     B2_KERNEL_CHECK();
@@ -697,10 +762,12 @@ int data_costs_qualities(b2tex_ctx *c, const b2tex_settings *st, b2tex_dc_info *
         B2_TRY(c->need_bits.zero(s));
     }
     if (nf) {
-        ScopedTimer tm(c, "k_cull<fill>", mesh_bytes + 6.0 * (double)num_cand);
-        B2_LAUNCH k_cull<true><<<blocks, 256, 0, s>>>(c->verts.p, c->faces.p, c->normals.p, c->views_dev.p, K, fb, fe,
-                                            cos_thr, nullptr, c->cand_ptr.p, c->cand_view.p, c->cand_face.p,
-                                            vis ? c->need_bits.p : nullptr, vwords, c->vrank.p, c->s_pass_bits.p, kwords);
+        // pass words + offsets read, candidates written; with the ray bitmaps also the face's vertex ranks
+        ScopedTimer tm(c, "k_cull<fill>", (4.0 * kwords + 8.0 + (vis ? 24.0 : 0.0)) * nf + 6.0 * (double)num_cand);
+        B2_LAUNCH k_cull<true><<<face_warp_blocks(c, nf), 256, 0, s>>>(c->verts.p, c->faces.p, c->normals.p, c->views_dev.p, K, fb, fe,
+                                                                        cos_thr, nullptr, c->cand_ptr.p, c->cand_view.p, c->cand_face.p,
+                                                                        vis ? c->need_bits.p : nullptr, vwords, c->vrank.p,
+                                                                        c->s_pass_bits.p, kwords);
     }
     B2_KERNEL_CHECK();
     unsigned long long *ray_count = reinterpret_cast<unsigned long long *>(c->scalars.p + 2);
