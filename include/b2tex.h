@@ -106,6 +106,12 @@ typedef struct {
     float residual[3];          /* |r| / |b| per colour channel at exit */
 } b2tex_local_seam_info;
 
+/* radial distortion of one view: line 2 of its MVE .cam file (generate_texture_views.cpp:138-146) */
+typedef struct {
+    float flen;      /* focal length normalised by the larger image side */
+    float dist[2];   /* dist[0] == 0: no distortion; dist[1] != 0: Bundler k2 k4 model; else VisualSFM with k = dist[0] */
+} b2tex_distortion;
+
 typedef struct b2tex_ctx b2tex_ctx;
 
 /* ---- lifetime ---- */
@@ -134,6 +140,13 @@ int b2tex_set_labels(b2tex_ctx *ctx, const uint32_t *labels);
 /* restrict this context to faces [face_begin, face_end) for the data-cost stage (multi-GPU shard);
  * default is all faces */
 int b2tex_set_face_range(b2tex_ctx *ctx, uint32_t face_begin, uint32_t face_end);
+/* Undistorts the resident images in place, as the reference does while it loads a .cam scene
+ * (generate_texture_views.cpp:154-162, MVE image_undistort_k2k4 / image_undistort_vsfm): every later stage reads the
+ * undistorted pixels.  d[num_views], num_views == the number of views set.  Views with dist[0] == 0 stay untouched;
+ * pixels whose source falls outside the image become 0 (and so may give the view a validity mask).  B2TEX_ERR_ARG if no
+ * views are set, num_views differs, or a view to undistort has a focal length that is not finite and positive.  Call it
+ * after b2tex_set_views and before the stages; results of earlier stages are discarded. */
+int b2tex_undistort_views(b2tex_ctx *ctx, const b2tex_distortion *d, uint32_t num_views);
 
 int b2tex_data_costs_run(b2tex_ctx *ctx, const b2tex_settings *settings, b2tex_dc_info *info);
 /* split form of the normalisation for sharded runs (calculate_data_costs.cpp:277-302):

@@ -24,7 +24,7 @@ EXPORTS = [
     "b2tex_create", "b2tex_destroy", "b2tex_last_error", "b2tex_free", "b2tex_device_synchronize",
     "b2tex_stream", "b2tex_launch_count", "b2tex_profile", "b2tex_profile_report",
     "b2tex_default_mrf_params", "b2tex_set_mesh", "b2tex_set_views", "b2tex_set_adjacency",
-    "b2tex_set_vertex_rings", "b2tex_set_data_costs", "b2tex_set_labels", "b2tex_set_face_range",
+    "b2tex_set_vertex_rings", "b2tex_set_data_costs", "b2tex_set_labels", "b2tex_set_face_range", "b2tex_undistort_views",
     "b2tex_data_costs_run", "b2tex_data_costs_qualities", "b2tex_data_costs_histogram",
     "b2tex_data_costs_normalize", "b2tex_data_costs_download", "b2tex_view_selection_run", "b2tex_view_selection_prepare",
     "b2tex_labels_download", "b2tex_mrf_init", "b2tex_mrf_iterate", "b2tex_mrf_energy", "b2tex_mrf_sample_forest",
@@ -40,6 +40,10 @@ class B2View(C.Structure):
     _fields_ = [("pos", C.c_float * 3), ("viewdir", C.c_float * 3), ("proj", C.c_float * 9),
                 ("w2c", C.c_float * 16), ("width", C.c_int32), ("height", C.c_int32),
                 ("rgb", C.c_void_p)]
+
+
+class B2Distortion(C.Structure):
+    _fields_ = [("flen", C.c_float), ("dist", C.c_float * 2)]
 
 
 class B2Settings(C.Structure):
@@ -175,6 +179,21 @@ class Context:
         imgs = scene.images if images is None else images
         self.set_views(make_views(scene.pos, scene.viewdir, scene.proj, scene.w2c, scene.width,
                                   scene.height, imgs), scene.num_views)
+
+    def undistort_views(self, flen, dist):
+        """Undistort the resident images in place, as the reference does for .cam views (b2tex_undistort_views).
+        flen[K]: focal lengths normalised by the larger image side; dist[K, 2]: .cam radial coefficients.  A view with
+        dist[v, 0] == 0 is left as it is; dist[v, 1] != 0 selects the Bundler k2 k4 model, otherwise VisualSFM's.
+        Call after set_views / set_scene and before the stages."""
+        flen = np.asarray(flen, np.float32).reshape(-1)
+        dist = np.asarray(dist, np.float32).reshape(-1, 2)
+        if len(flen) != len(dist):
+            raise ValueError(f"undistort_views: {len(flen)} focal lengths for {len(dist)} distortions")
+        d = (B2Distortion * max(len(flen), 1))()
+        for v in range(len(flen)):
+            d[v].flen = float(flen[v])
+            d[v].dist[:] = dist[v].tolist()
+        _check(lib().b2tex_undistort_views(self._h, d, C.c_uint32(len(flen))))
 
     def set_adjacency(self, adj_ptr, adj_idx):
         _check(lib().b2tex_set_adjacency(self._h, _p(_c(adj_ptr, np.uint32)), _p(_c(adj_idx, np.uint32))))

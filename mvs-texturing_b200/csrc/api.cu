@@ -184,6 +184,12 @@ int b2tex_set_views(b2tex_ctx *c, const b2tex_view *views, uint32_t K)
     return B2TEX_OK;
 }
 
+int b2tex_undistort_views(b2tex_ctx *c, const b2tex_distortion *d, uint32_t num_views)
+{
+    B2_CUDA(cudaSetDevice(c->device));
+    return undistort_views(c, d, num_views);
+}
+
 int b2tex_set_adjacency(b2tex_ctx *c, const uint32_t *adj_ptr, const uint32_t *adj_idx)
 {
     B2_CUDA(cudaSetDevice(c->device));

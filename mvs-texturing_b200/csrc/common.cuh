@@ -269,6 +269,9 @@ struct ScopedTimer {
 int prepare_images(b2tex_ctx *c, int data_term, bool force = false);
 int prepare_views(b2tex_ctx *c, int data_term);    // camera block only (no pixel data needed)
 int wait_for_images(b2tex_ctx *c);                 // the compute stream waits for a deferred image upload
+// flags[v] != 0: view v has a zero-sum corner pixel (it gets a validity mask); reads the camera block in views_dev
+int zero_corner_flags(b2tex_ctx *c, std::vector<uint32_t> &flags);
+int undistort_views(b2tex_ctx *c, const b2tex_distortion *d, uint32_t num_views);
 int build_bvh(b2tex_ctx *c, bool force = false);
 int data_costs_qualities(b2tex_ctx *c, const b2tex_settings *st, b2tex_dc_info *info);
 int data_costs_histogram(b2tex_ctx *c, float gmax);

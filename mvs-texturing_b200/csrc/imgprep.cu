@@ -304,21 +304,36 @@ __global__ void k_corner_check(const ViewDev *views, int K, uint32_t *flags)
     flags[v] = any;
 }
 
-__global__ void k_flood_seed(const uint8_t *rgb, uint8_t *inv, int w, int h)
+// one view of a batched flood: its image and its invalid map (1 = invalid)
+struct FloodView {
+    const uint8_t *rgb;
+    uint8_t *inv;
+    int32_t w, h;
+};
+
+// thread per (view, corner)
+__global__ void k_flood_seed(const FloodView *__restrict__ views, uint32_t n)
 {
-    int i = threadIdx.x;
-    if (i >= 4) return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 4 * n) return;
+    const FloodView V = views[i >> 2];
+    const int w = V.w, h = V.h;
     int cx = (i & 2) ? w - 1 : 0, cy = (i & 1) ? h - 1 : 0;
-    const uint8_t *p = rgb + 3 * ((size_t)cx + (size_t)cy * w);
-    if ((int)p[0] + p[1] + p[2] == 0) inv[(size_t)cx + (size_t)cy * w] = 1;
+    const uint8_t *p = V.rgb + 3 * ((size_t)cx + (size_t)cy * w);
+    if ((int)p[0] + p[1] + p[2] == 0) V.inv[(size_t)cx + (size_t)cy * w] = 1;
 }
 
-// tile-local flood iteration: invalid spreads through 4-connected zero-sum pixels
-__global__ void __launch_bounds__(256) k_flood(const uint8_t *__restrict__ rgb, uint8_t *inv, int w,
-                                               int h, uint32_t *changed)
+// tile-local flood iteration over a batch of views (blockIdx.z = view): invalid spreads through 4-connected zero-sum
+// pixels; any block that marked a pixel sets *changed
+__global__ void __launch_bounds__(256) k_flood(const FloodView *__restrict__ views, uint32_t *changed)
 {
     __shared__ uint8_t z[34][36], s[34][36];
+    const FloodView V = views[blockIdx.z];
+    const uint8_t *__restrict__ rgb = V.rgb;
+    uint8_t *inv = V.inv;
+    const int w = V.w, h = V.h;
     const int x0 = blockIdx.x * 32, y0 = blockIdx.y * 32;
+    if (x0 >= w || y0 >= h) return;   // the grid covers the largest view of the batch; the whole block leaves
     for (int i = threadIdx.x; i < 34 * 34; i += blockDim.x) {
         int ly = i / 34, lx = i - ly * 34;
         int gx = x0 + lx - 1, gy = y0 + ly - 1;
@@ -389,6 +404,50 @@ int wait_for_images(b2tex_ctx *c)
     if (c->images_in_flight) {
         B2_CUDA(cudaStreamWaitEvent(c->stream, c->images_uploaded, 0));
         c->images_in_flight = false;
+    }
+    return B2TEX_OK;
+}
+
+int zero_corner_flags(b2tex_ctx *c, std::vector<uint32_t> &flags)
+{
+    cudaStream_t s = c->stream;
+    const uint32_t K = c->K;
+    B2_TRY(c->scalars.alloc(std::max<size_t>(K + 64, 256)));
+    B2_LAUNCH k_corner_check<<<(K + 127) / 128, 128, 0, s>>>(c->views_dev.p, (int)K, c->scalars.p + 64);
+    B2_KERNEL_CHECK();
+    flags.assign(K, 0);
+    B2_CUDA(cudaMemcpyAsync(flags.data(), c->scalars.p + 64, K * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    B2_CUDA(cudaStreamSynchronize(s));
+    return B2TEX_OK;
+}
+
+// Corner flood of the views fv (zeroed invalid maps): rounds of k_flood until no block marks a pixel.  One round covers
+// up to B2TEX_FLOOD_BATCH views (default: all) in one launch with one change counter and one host poll; the fixpoint,
+// and so every mask, does not depend on how the views are batched.  B2TEX_FLOOD_BATCH=1 floods view after view
+// (diagnostic: it is what the batched rounds are measured against).
+static int flood_fill(b2tex_ctx *c, const std::vector<FloodView> &fv, const FloodView *fv_dev)
+{
+    cudaStream_t s = c->stream;
+    const size_t n = fv.size();
+    size_t batch = n;
+    if (const char *e = getenv("B2TEX_FLOOD_BATCH")) batch = std::max<size_t>(1, std::min<size_t>(n, strtoull(e, nullptr, 10)));
+    batch = std::min<size_t>(batch, 65535);   // gridDim.z
+    ScopedTimer tm(c, "k_flood", 0.0);
+    for (size_t i0 = 0; i0 < n; i0 += batch) {
+        const size_t nb = std::min(batch, n - i0);
+        int maxw = 0, maxh = 0;
+        for (size_t i = i0; i < i0 + nb; ++i) { maxw = std::max(maxw, (int)fv[i].w); maxh = std::max(maxh, (int)fv[i].h); }
+        B2_LAUNCH k_flood_seed<<<(unsigned)((4 * nb + 127) / 128), 128, 0, s>>>(fv_dev + i0, (uint32_t)nb);
+        const dim3 fgrid((maxw + 31) / 32, (maxh + 31) / 32, (unsigned)nb);
+        for (int it = 0; it < 100000; ++it) {
+            B2_CUDA(cudaMemsetAsync(c->scalars.p, 0, sizeof(uint32_t), s));
+            B2_LAUNCH k_flood<<<fgrid, 256, 0, s>>>(fv_dev + i0, c->scalars.p);
+            uint32_t changed = 0;
+            B2_CUDA(cudaMemcpyAsync(&changed, c->scalars.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+            B2_CUDA(cudaStreamSynchronize(s));
+            if (!changed) break;
+        }
+        B2_KERNEL_CHECK();
     }
     return B2TEX_OK;
 }
@@ -486,46 +545,36 @@ int prepare_images(b2tex_ctx *c, int data_term, bool force)
     std::vector<ViewDev> vd;
     fill_view_block(c, data_term, vd);
     B2_TRY(c->views_dev.upload(vd.data(), K, s));
-    B2_TRY(c->scalars.alloc(std::max<size_t>(K + 64, 256)));
-    B2_LAUNCH k_corner_check<<<(K + 127) / 128, 128, 0, s>>>(c->views_dev.p, (int)K, c->scalars.p + 64);
-    B2_KERNEL_CHECK();
-    std::vector<uint32_t> flags(K);
-    B2_CUDA(cudaMemcpyAsync(flags.data(), c->scalars.p + 64, K * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    B2_CUDA(cudaStreamSynchronize(s));
-    bool any = false;
-    for (uint32_t v = 0; v < K; ++v) any |= flags[v] != 0;
-    if (any) {
+    std::vector<uint32_t> flags;
+    B2_TRY(zero_corner_flags(c, flags));
+    std::vector<FloodView> fv;
+    size_t maxpx = 0;
+    for (uint32_t v = 0; v < K; ++v) {
+        if (!flags[v]) continue;
+        // the flood runs in the view's slot of valid4, which k_valid4 overwrites at the end
+        fv.push_back({c->rgb.p + 3 * c->img_off[v], nullptr, c->views_host[v].width, c->views_host[v].height});
+        maxpx = std::max(maxpx, (size_t)c->views_host[v].width * c->views_host[v].height);
+    }
+    if (!fv.empty()) {
         B2_TRY(c->valid4.alloc(total_px));
-        DevBuf<uint8_t> inv, er;
-        size_t maxpx = 0;
-        for (uint32_t v = 0; v < K; ++v)
-            maxpx = std::max(maxpx, (size_t)c->views_host[v].width * c->views_host[v].height);
-        B2_TRY(inv.alloc(maxpx));
+        for (uint32_t v = 0, i = 0; v < K; ++v)
+            if (flags[v]) fv[i++].inv = c->valid4.p + c->img_off[v];
+        for (const FloodView &f : fv) B2_CUDA(cudaMemsetAsync(f.inv, 0, (size_t)f.w * f.h, s));
+        DevBuf<FloodView> fv_dev;
+        B2_TRY(fv_dev.upload(fv.data(), fv.size(), s));
+        B2_TRY(flood_fill(c, fv, fv_dev.p));
+        DevBuf<uint8_t> er;
         B2_TRY(er.alloc(maxpx));
         for (uint32_t v = 0; v < K; ++v) {
             if (!flags[v]) continue;
             int w = c->views_host[v].width, h = c->views_host[v].height;
-            const uint8_t *rgb = c->rgb.p + 3 * c->img_off[v];
-            B2_CUDA(cudaMemsetAsync(inv.p, 0, (size_t)w * h, s));
-            B2_LAUNCH k_flood_seed<<<1, 32, 0, s>>>(rgb, inv.p, w, h);
-            dim3 fgrid((w + 31) / 32, (h + 31) / 32);
-            for (int it = 0; it < 100000; ++it) {
-                B2_CUDA(cudaMemsetAsync(c->scalars.p, 0, sizeof(uint32_t), s));
-                B2_LAUNCH k_flood<<<fgrid, 256, 0, s>>>(rgb, inv.p, w, h, c->scalars.p);
-                uint32_t changed = 0;
-                B2_CUDA(cudaMemcpyAsync(&changed, c->scalars.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-                B2_CUDA(cudaStreamSynchronize(s));
-                if (!changed) break;
-            }
+            uint8_t *inv = c->valid4.p + c->img_off[v];
             dim3 b(32, 8), g((w + 31) / 32, (h + 7) / 8);
-            const uint8_t *src = inv.p;
-            if (data_term == 1) {
-                B2_LAUNCH k_erode<<<g, b, 0, s>>>(inv.p, er.p, w, h);
-                src = er.p;
-            }
-            B2_LAUNCH k_valid4<<<g, b, 0, s>>>(src, c->valid4.p + c->img_off[v], w, h);
+            if (data_term == 1) B2_LAUNCH k_erode<<<g, b, 0, s>>>(inv, er.p, w, h);
+            else B2_CUDA(cudaMemcpyAsync(er.p, inv, (size_t)w * h, cudaMemcpyDeviceToDevice, s));
+            B2_LAUNCH k_valid4<<<g, b, 0, s>>>(er.p, inv, w, h);
             B2_KERNEL_CHECK();
-            vd[v].valid4 = c->valid4.p + c->img_off[v];
+            vd[v].valid4 = inv;
         }
         B2_CUDA(cudaStreamSynchronize(s));
         B2_TRY(c->views_dev.upload(vd.data(), K, s));

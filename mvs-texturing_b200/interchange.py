@@ -134,7 +134,8 @@ def load_cam(filename, width, height):
     line 2 = focal length [dist0 dist1 pixel aspect principal x y].  Returns the four quantities TextureView keeps
     (texture_view.cpp:33-39): pos, viewdir, proj (3x3, pixels), world_to_cam (4x4).  mve::CameraInfo's fill_* are
     restated [UPSTREAM-RECALL]: pos = -R^T t, viewdir = third row of R, calibration scaled by the larger image side.
-    Undistortion (dist != 0, :139-151) is not applied here."""
+    Undistortion (dist != 0, :152-162) is not applied here: pass flen and dist to Context.undistort_views after the
+    images are set."""
     try:
         with open(filename) as f:
             ext = f.readline().split()
