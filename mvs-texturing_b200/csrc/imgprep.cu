@@ -6,7 +6,6 @@
 //   valid4             = AND of the 4 bilinear taps          (texture_view.cpp:264-277)
 // Integer/u8 outputs are bit-exact restatements; compiled with -fmad=false.
 #include <cuda.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -14,114 +13,92 @@ namespace b2 {
 
 namespace {
 
-constexpr int TW = 64, TH = 16;
-
-__device__ __forceinline__ uint8_t luminance_u8(const uint8_t *px)
+// ---- gradient magnitude: the arithmetic both gradient kernels share, and the kernel for views of any size -------------
+// MVE desaturate_luminance -> math::interpolate<uchar>: (u8)(r*.21f + g*.72f + b*.07f + .5f)
+__device__ __forceinline__ uint8_t luminance_u8(uint32_t r, uint32_t g, uint32_t b)
 {
-    // MVE desaturate_luminance -> math::interpolate<uchar>: (u8)(r*.21f + g*.72f + b*.07f + .5f)
-    float v = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn((float)px[0], 0.21f), __fmul_rn((float)px[1], 0.72f)),
-                                  __fmul_rn((float)px[2], 0.07f)), 0.5f);
-    return (uint8_t)v;
+    return (uint8_t)__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn((float)r, 0.21f), __fmul_rn((float)g, 0.72f)), __fmul_rn((float)b, 0.07f)),
+                              0.5f);
 }
 
-// One block = TW x TH output pixels; luminance tile with a 1-pixel halo staged in shared memory so
-// every rgb byte is read once from global (HBM-bound: 3 B read + 1 B written per pixel).
-__global__ void __launch_bounds__(256) k_lum_sobel(const uint8_t *__restrict__ rgb,
-                                                   uint8_t *__restrict__ grad, int w, int h)
+// (u8)min(255, sqrt(sx^2 + sy^2)) of the integer Sobel sums.  ss < 2^24 is exact in fp32, and for ss < 255^2 the correctly
+// rounded fp32 root of an integer cannot round up to the next integer (k - sqrt(k^2-1) > 1/(2k) >> ulp): its truncation
+// is floor(sqrt(ss)), as the oracle's double root gives
+__device__ __forceinline__ uint32_t sobel_u8(int sx, int sy)
 {
-    __shared__ uint8_t lum[TH + 2][TW + 2 + 2];
+    const int ss = sx * sx + sy * sy;
+    return ss >= 255 * 255 ? 255u : (uint32_t)(int)__fsqrt_rn((float)ss);
+}
+
+// one view of a batched gradient: its image and its gradient magnitude
+struct GradView {
+    const uint8_t *rgb;
+    uint8_t *grad;
+    int32_t w, h;
+};
+
+// Gradient of views of any size, all in one launch (blockIdx.z = view; the grid covers the largest view).  One block =
+// TW x TH output pixels.  The raw rgb rows of the tile and its 1-pixel halo are staged with aligned 32-bit loads
+// (coalesced; byte loads move 3 B per thread and reach <10 % of HBM peak); a row starts at any byte, so each staged row
+// keeps the offset of its first byte in its first word.  Only the view's own bytes [rgb, rgb + 3 w h) are read: a word
+// that lies partly outside them is read byte by byte.  Luminance is computed from shared memory, and the gradient
+// leaves as 32-bit words where the row is aligned.  32 rows per block pay the view-table load and the halo rows once
+// for twice the pixels of 16 rows, which measured 4 % slower on 200 views at 1912x1080.
+constexpr int TW = 128, TH = 32, RW = (3 * (TW + 2) + 3 + 3) / 4 + 1;
+__global__ void __launch_bounds__(256) k_lum_sobel(const GradView *__restrict__ views)
+{
+    __shared__ uint32_t raw[TH + 2][RW];
+    __shared__ uint8_t lum[TH + 2][TW + 4];
+    __shared__ uint32_t shift_s[TH + 2];
+    const GradView V = views[blockIdx.z];
+    const int w = V.w, h = V.h;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
-    for (int i = threadIdx.x; i < (TW + 2) * (TH + 2); i += blockDim.x) {
-        int ly = i / (TW + 2), lx = i - ly * (TW + 2);
-        int gx = x0 + lx - 1, gy = y0 + ly - 1;
-        uint8_t v = 0;
-        if (gx >= 0 && gx < w && gy >= 0 && gy < h) v = luminance_u8(rgb + 3 * ((size_t)gx + (size_t)gy * w));
-        lum[ly][lx] = v;
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < TW * TH; i += blockDim.x) {
-        int ly = i / TW, lx = i - ly * TW;
-        int gx = x0 + lx, gy = y0 + ly;
-        if (gx >= w || gy >= h) continue;
-        uint8_t out = 0;
-        if (!(gy == 0 || gy == h - 1 || gx == 0 || gx == w - 1)) {
-            int a = lum[ly][lx], b = lum[ly][lx + 1], c = lum[ly][lx + 2];
-            int d = lum[ly + 1][lx], f = lum[ly + 1][lx + 2];
-            int g = lum[ly + 2][lx], hh = lum[ly + 2][lx + 1], k = lum[ly + 2][lx + 2];
-            int sx = (c - a) + 2 * (f - d) + (k - g);
-            int sy = (g - a) + 2 * (hh - b) + (k - c);
-            int s = sx * sx + sy * sy;  // exact; (u8)min(255, sqrt(double(s))) == min(255, isqrt(s))
-            int r = (int)sqrtf((float)s);
-            while (r * r > s) --r;
-            while ((r + 1) * (r + 1) <= s) ++r;
-            out = (uint8_t)(r < 255 ? r : 255);
-        }
-        grad[(size_t)gx + (size_t)gy * w] = out;
-    }
-}
-
-// Vectorised variant used for the whole view set in ONE launch (blockIdx.z = view): raw rgb rows are
-// staged with aligned 32-bit loads (coalesced; the byte-granular version above moves 3 B per thread and
-// reaches <10 % of HBM peak), luminance is computed from shared memory, and the gradient is written
-// as 32-bit words.  Arithmetic is identical (bit-exact u8 results).
-constexpr int TW2 = 128, TH2 = 16, RW2 = (3 * (TW2 + 2) + 3 + 3) / 4 + 1;
-__global__ void __launch_bounds__(256) k_lum_sobel_vec(const uint8_t *__restrict__ rgb_all,
-                                                       uint8_t *__restrict__ grad_all, int w, int h,
-                                                       size_t view_stride_px, const uint8_t *alloc_begin,
-                                                       const uint8_t *alloc_end)
-{
-    __shared__ uint32_t raw[TH2 + 2][RW2];
-    __shared__ uint8_t lum[TH2 + 2][TW2 + 4];
-    __shared__ uint32_t shift_s[TH2 + 2];
-    const uint8_t *rgb = rgb_all + 3 * view_stride_px * blockIdx.z;
-    uint8_t *grad = grad_all + view_stride_px * blockIdx.z;
-    const int x0 = blockIdx.x * TW2, y0 = blockIdx.y * TH2;
-    for (int i = threadIdx.x; i < (TH2 + 2) * RW2; i += blockDim.x) {
-        const int ly = i / RW2, wi = i - ly * RW2;
+    if (x0 >= w || y0 >= h) return;   // the whole block leaves
+    const uintptr_t lo = (uintptr_t)V.rgb, hi = lo + 3 * (size_t)w * h;
+    for (int i = threadIdx.x; i < (TH + 2) * RW; i += blockDim.x) {
+        const int ly = i / RW, wi = i - ly * RW;
         const int gy = y0 + ly - 1;
+        if (gy < 0 || gy >= h) continue;   // rows outside the view are never read
+        const uintptr_t a = lo + (size_t)gy * w * 3 + (intptr_t)(3 * (x0 - 1));
+        const uintptr_t al = a & ~(uintptr_t)3, wp = al + 4 * (uintptr_t)wi;
+        if (wi == 0) shift_s[ly] = (uint32_t)(a - al);
         uint32_t v = 0;
-        if (gy >= 0 && gy < h) {
-            const uintptr_t a = (uintptr_t)(rgb + (size_t)gy * w * 3) + (intptr_t)(3 * (x0 - 1));
-            const uintptr_t al = a & ~(uintptr_t)3;
-            if (wi == 0) shift_s[ly] = (uint32_t)(a - al);
-            const uint8_t *wp = (const uint8_t *)(al + 4 * (uintptr_t)wi);
-            if (wp >= alloc_begin && wp + 4 <= alloc_end) v = __ldg((const uint32_t *)wp);
-        } else if (wi == 0) shift_s[ly] = 0;
+        if (wp >= lo && wp + 4 <= hi)
+            v = __ldg((const uint32_t *)wp);
+        else
+            for (int j = 0; j < 4; ++j)
+                if (wp + j >= lo && wp + j < hi) v |= (uint32_t)__ldg((const uint8_t *)(wp + j)) << (8 * j);
         raw[ly][wi] = v;
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < (TH2 + 2) * (TW2 + 2); i += blockDim.x) {
-        const int ly = i / (TW2 + 2), lx = i - ly * (TW2 + 2);
+    for (int i = threadIdx.x; i < (TH + 2) * (TW + 2); i += blockDim.x) {
+        const int ly = i / (TW + 2), lx = i - ly * (TW + 2);
         const int gx = x0 + lx - 1, gy = y0 + ly - 1;
-        uint8_t v = 0;
-        if (gx >= 0 && gx < w && gy >= 0 && gy < h)
-            v = luminance_u8(reinterpret_cast<const uint8_t *>(raw[ly]) + shift_s[ly] + 3 * lx);
+        uint8_t v = 0;   // luminance 0 outside the image
+        if (gx >= 0 && gx < w && gy >= 0 && gy < h) {
+            const uint8_t *p = reinterpret_cast<const uint8_t *>(raw[ly]) + shift_s[ly] + 3 * lx;
+            v = luminance_u8(p[0], p[1], p[2]);
+        }
         lum[ly][lx] = v;
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < TW2 * TH2 / 4; i += blockDim.x) {
-        const int ly = i / (TW2 / 4), lx0 = (i - ly * (TW2 / 4)) * 4;
+    for (int i = threadIdx.x; i < TW * TH / 4; i += blockDim.x) {
+        const int ly = i / (TW / 4), lx0 = (i - ly * (TW / 4)) * 4;
         const int gy = y0 + ly;
         if (gy >= h) continue;
         uint8_t o[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int lx = lx0 + j, gx = x0 + lx;
-            uint8_t out = 0;
+            o[j] = 0;
             if (gx < w && !(gy == 0 || gy == h - 1 || gx == 0 || gx == w - 1)) {
-                int a = lum[ly][lx], b = lum[ly][lx + 1], c = lum[ly][lx + 2];
-                int d = lum[ly + 1][lx], f = lum[ly + 1][lx + 2];
-                int g = lum[ly + 2][lx], hh = lum[ly + 2][lx + 1], k = lum[ly + 2][lx + 2];
-                int sx = (c - a) + 2 * (f - d) + (k - g);
-                int sy = (g - a) + 2 * (hh - b) + (k - c);
-                const int ss = sx * sx + sy * sy;  // < 2^24: exact in fp32
-                // floor(sqrt(ss)) for ss < 255^2: the correctly rounded fp32 root of an integer below
-                // 2^16 cannot round up to the next integer (k - sqrt(k^2-1) > 1/(2k) >> ulp)
-                out = ss >= 255 * 255 ? (uint8_t)255 : (uint8_t)(int)__fsqrt_rn((float)ss);
+                const int a = lum[ly][lx], b = lum[ly][lx + 1], c = lum[ly][lx + 2];
+                const int d = lum[ly + 1][lx], f = lum[ly + 1][lx + 2];
+                const int g = lum[ly + 2][lx], hh = lum[ly + 2][lx + 1], k = lum[ly + 2][lx + 2];
+                o[j] = (uint8_t)sobel_u8((c - a) + 2 * (f - d) + (k - g), (g - a) + 2 * (hh - b) + (k - c));
             }
-            o[j] = out;
         }
-        uint8_t *dst = grad + (size_t)gy * w + x0 + lx0;
+        uint8_t *dst = V.grad + (size_t)gy * w + x0 + lx0;
         if (x0 + lx0 + 3 < w && (((uintptr_t)dst) & 3) == 0) {
             *reinterpret_cast<uint32_t *>(dst) = (uint32_t)o[0] | ((uint32_t)o[1] << 8) | ((uint32_t)o[2] << 16) | ((uint32_t)o[3] << 24);
         } else {
@@ -131,7 +108,6 @@ __global__ void __launch_bounds__(256) k_lum_sobel_vec(const uint8_t *__restrict
     }
 }
 
-
 // ---- TMA variant: the rgb tile (+ 1 pixel halo) of a view is staged by ONE bulk tensor copy ------------------------------
 // The view set is described to the TMA unit as a 3-D tensor of 32-bit words [K][H][3 W / 4] (needs W % 16 == 0: global
 // strides are multiples of 16 bytes); a CTA asks for the box {104 words, TH3 + 2 rows, 1 view} that holds the
@@ -139,8 +115,8 @@ __global__ void __launch_bounds__(256) k_lum_sobel_vec(const uint8_t *__restrict
 // load.  Two rules keep every box to what the TMA unit accepts: the first
 // coordinate of the box starts on a 16-byte boundary of the row, so
 // the box starts three words early (104 words instead of 100); and the box of an edge tile is shifted back inside the
-// image instead of relying on out-of-bounds fill, the out-of-image pixels get luminance 0 explicitly, which is what the
-// scalar kernel assigns there.  Luminance is then computed four pixels per thread from 16-byte windows of
+// image instead of relying on out-of-bounds fill, the out-of-image pixels get luminance 0 explicitly, as k_lum_sobel
+// gives them.  Luminance is then computed four pixels per thread from 16-byte windows of
 // the raw tile, the Sobel sums four outputs per thread from six 32-bit words of the luminance tile with shared column
 // and row sums, and the gradient leaves as one 32-bit word per thread.  Same integer / fp32 arithmetic, bit-exact.
 constexpr int TW3 = 128, TH3 = 32;
@@ -148,8 +124,9 @@ constexpr int BOXW3 = 104;                 // words per tile row: bytes [384 bx 
 constexpr int LUMW3 = 136;                 // luminance tile row pitch (132 pixels used)
 __device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void lum_sobel_tma_body(const CUtensorMap *tmap, uint8_t *__restrict__ grad_all,
-                                                   int w, int h, size_t view_stride_px, uint32_t *timeouts)
+// The 128-byte descriptor lives in global memory.
+__global__ void __launch_bounds__(256) k_lum_sobel_tma(const CUtensorMap *__restrict__ tmap, uint8_t *__restrict__ grad_all,
+                                                       int w, int h, size_t view_stride_px, uint32_t *timeouts)
 {
     __shared__ __align__(128) uint32_t raw[(TH3 + 2) * BOXW3];
     __shared__ __align__(16) uint8_t lum[(TH3 + 2) * LUMW3];
@@ -204,9 +181,7 @@ __device__ __forceinline__ void lum_sobel_tma_body(const CUtensorMap *tmap, uint
                     const uint32_t word = o < 4 ? w0 : (o < 8 ? w1 : (o < 12 ? w2 : w3));
                     return (word >> (8 * (o & 3))) & 0xFFu;
                 };
-                const float v = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn((float)byte_at(b), 0.21f), __fmul_rn((float)byte_at(b + 1), 0.72f)),
-                                                    __fmul_rn((float)byte_at(b + 2), 0.07f)), 0.5f);
-                out |= ((uint32_t)(uint8_t)v) << (8 * q);
+                out |= (uint32_t)luminance_u8(byte_at(b), byte_at(b + 1), byte_at(b + 2)) << (8 * q);
             }
         }
         *reinterpret_cast<uint32_t *>(lum + ly * LUMW3 + 4 * j) = out;
@@ -238,30 +213,15 @@ __device__ __forceinline__ void lum_sobel_tma_body(const CUtensorMap *tmap, uint
         for (int q = 0; q < 4; ++q) {
             const int gx = gx0 + q;
             uint32_t out = 0;
-            if (gx < w && !(gy == 0 || gy == h - 1 || gx == 0 || gx == w - 1)) {
-                const int sx = col[q + 2] - col[q];   // (c - a) + 2 (f - d) + (k - g)
-                const int sy = rowb[q] - rowt[q];     // (g - a) + 2 (hh - b) + (k - c)
-                const int ss = sx * sx + sy * sy;     // < 2^24: exact in fp32
-                out = ss >= 255 * 255 ? 255u : (uint32_t)(int)__fsqrt_rn((float)ss);
-            }
+            if (gx < w && !(gy == 0 || gy == h - 1 || gx == 0 || gx == w - 1))
+                out = sobel_u8(col[q + 2] - col[q],    // (c - a) + 2 (f - d) + (k - g)
+                               rowb[q] - rowt[q]);     // (g - a) + 2 (hh - b) + (k - c)
             o |= out << (8 * q);
         }
         uint8_t *dst = grad + (size_t)gy * w + gx0;
         if (gx0 + 3 < w) *reinterpret_cast<uint32_t *>(dst) = o;   // w % 16 == 0 and gx0 % 4 == 0: aligned
         else for (int q = 0; q < 4 && gx0 + q < w; ++q) dst[q] = (uint8_t)(o >> (8 * q));
     }
-}
-
-// the descriptor either in global memory or (B2TEX_TMA_MODE=2) as a __grid_constant__ kernel parameter
-__global__ void __launch_bounds__(256) k_lum_sobel_tma(const CUtensorMap *__restrict__ tmap, uint8_t *__restrict__ grad_all,
-                                                       int w, int h, size_t view_stride_px, uint32_t *timeouts)
-{
-    lum_sobel_tma_body(tmap, grad_all, w, h, view_stride_px, timeouts);
-}
-__global__ void __launch_bounds__(256) k_lum_sobel_tma_param(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ grad_all,
-                                                             int w, int h, size_t view_stride_px, uint32_t *timeouts)
-{
-    lum_sobel_tma_body(&tmap, grad_all, w, h, view_stride_px, timeouts);
 }
 
 // the tensor map of the rgb images of a uniform view set, or false if the layout does not qualify
@@ -421,34 +381,27 @@ int zero_corner_flags(b2tex_ctx *c, std::vector<uint32_t> &flags)
     return B2TEX_OK;
 }
 
-// Corner flood of the views fv (zeroed invalid maps): rounds of k_flood until no block marks a pixel.  One round covers
-// up to B2TEX_FLOOD_BATCH views (default: all) in one launch with one change counter and one host poll; the fixpoint,
-// and so every mask, does not depend on how the views are batched.  B2TEX_FLOOD_BATCH=1 floods view after view
-// (diagnostic: it is what the batched rounds are measured against).
+// Corner flood of the views fv (zeroed invalid maps): rounds of k_flood over all of them, each round one launch with one
+// change counter and one host poll, until no block marks a pixel.  fv.size() <= K <= 65535 (b2tex_set_views), the limit
+// of gridDim.z.
 static int flood_fill(b2tex_ctx *c, const std::vector<FloodView> &fv, const FloodView *fv_dev)
 {
     cudaStream_t s = c->stream;
-    const size_t n = fv.size();
-    size_t batch = n;
-    if (const char *e = getenv("B2TEX_FLOOD_BATCH")) batch = std::max<size_t>(1, std::min<size_t>(n, strtoull(e, nullptr, 10)));
-    batch = std::min<size_t>(batch, 65535);   // gridDim.z
+    const uint32_t n = (uint32_t)fv.size();
+    int maxw = 0, maxh = 0;
+    for (const FloodView &f : fv) { maxw = std::max(maxw, (int)f.w); maxh = std::max(maxh, (int)f.h); }
     ScopedTimer tm(c, "k_flood", 0.0);
-    for (size_t i0 = 0; i0 < n; i0 += batch) {
-        const size_t nb = std::min(batch, n - i0);
-        int maxw = 0, maxh = 0;
-        for (size_t i = i0; i < i0 + nb; ++i) { maxw = std::max(maxw, (int)fv[i].w); maxh = std::max(maxh, (int)fv[i].h); }
-        B2_LAUNCH k_flood_seed<<<(unsigned)((4 * nb + 127) / 128), 128, 0, s>>>(fv_dev + i0, (uint32_t)nb);
-        const dim3 fgrid((maxw + 31) / 32, (maxh + 31) / 32, (unsigned)nb);
-        for (int it = 0; it < 100000; ++it) {
-            B2_CUDA(cudaMemsetAsync(c->scalars.p, 0, sizeof(uint32_t), s));
-            B2_LAUNCH k_flood<<<fgrid, 256, 0, s>>>(fv_dev + i0, c->scalars.p);
-            uint32_t changed = 0;
-            B2_CUDA(cudaMemcpyAsync(&changed, c->scalars.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-            B2_CUDA(cudaStreamSynchronize(s));
-            if (!changed) break;
-        }
-        B2_KERNEL_CHECK();
+    B2_LAUNCH k_flood_seed<<<(4 * n + 127) / 128, 128, 0, s>>>(fv_dev, n);
+    const dim3 fgrid((maxw + 31) / 32, (maxh + 31) / 32, n);
+    for (int it = 0; it < 100000; ++it) {
+        B2_CUDA(cudaMemsetAsync(c->scalars.p, 0, sizeof(uint32_t), s));
+        B2_LAUNCH k_flood<<<fgrid, 256, 0, s>>>(fv_dev, c->scalars.p);
+        uint32_t changed = 0;
+        B2_CUDA(cudaMemcpyAsync(&changed, c->scalars.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        B2_CUDA(cudaStreamSynchronize(s));
+        if (!changed) break;
     }
+    B2_KERNEL_CHECK();
     return B2TEX_OK;
 }
 
@@ -493,31 +446,22 @@ int prepare_images(b2tex_ctx *c, int data_term, bool force)
 
     if (data_term == 1) {
         B2_TRY(c->grad.alloc(total_px));
+        DevBuf<GradView> gv_dev;   // k_lum_sobel's view table; freed after the timer has stopped
         ScopedTimer tm(c, "k_lum_sobel", 4.0 * (double)total_px);  // 3 B rgb read + 1 B gradient written
+        const int w = c->views_host[0].width, h = c->views_host[0].height;
         bool uniform = true;
-        for (uint32_t v = 1; v < K; ++v)
-            uniform = uniform && c->views_host[v].width == c->views_host[0].width
-                && c->views_host[v].height == c->views_host[0].height;
-        static const bool scalar_sobel = getenv("B2TEX_SCALAR_SOBEL") != nullptr;
-        // B2TEX_TMA=0 switches the TMA-staged kernel off (diagnostic)
-        static const bool use_tma = !(getenv("B2TEX_TMA") && atoi(getenv("B2TEX_TMA")) == 0) && getenv("B2TEX_NO_TMA") == nullptr;
+        for (uint32_t v = 1; v < K; ++v) uniform = uniform && c->views_host[v].width == w && c->views_host[v].height == h;
         alignas(64) CUtensorMap tmap;
-        if (uniform && K <= 65535u && !scalar_sobel && use_tma &&
-            make_rgb_tensor_map(c->rgb.p, c->views_host[0].width, c->views_host[0].height, K, &tmap)) {
+        if (uniform && make_rgb_tensor_map(c->rgb.p, w, h, K, &tmap)) {
             // image tiles staged by the TMA unit (one bulk tensor copy per CTA), all views in one launch.  The 128-byte
             // descriptor lives in global memory (64-byte aligned), next to a counter of copies that never arrived.
-            int w = c->views_host[0].width, h = c->views_host[0].height;
             B2_TRY(c->tmap_dev.alloc(256));
             B2_CUDA(cudaMemcpyAsync(c->tmap_dev.p, &tmap, sizeof(tmap), cudaMemcpyHostToDevice, s));
             B2_CUDA(cudaMemsetAsync(c->tmap_dev.p + 128, 0, 4, s));
             B2_CUDA(cudaStreamSynchronize(s));   // tmap is a local
             dim3 grid((w + TW3 - 1) / TW3, (h + TH3 - 1) / TH3, K);
-            static const int tma_mode = getenv("B2TEX_TMA_MODE") ? atoi(getenv("B2TEX_TMA_MODE")) : 1;
-            if (tma_mode == 2)
-                B2_LAUNCH k_lum_sobel_tma_param<<<grid, 256, 0, s>>>(tmap, c->grad.p, w, h, (size_t)w * h, reinterpret_cast<uint32_t *>(c->tmap_dev.p + 128));
-            else
-                B2_LAUNCH k_lum_sobel_tma<<<grid, 256, 0, s>>>(reinterpret_cast<const CUtensorMap *>(c->tmap_dev.p), c->grad.p, w, h, (size_t)w * h,
-                                                     reinterpret_cast<uint32_t *>(c->tmap_dev.p + 128));
+            B2_LAUNCH k_lum_sobel_tma<<<grid, 256, 0, s>>>(reinterpret_cast<const CUtensorMap *>(c->tmap_dev.p), c->grad.p, w, h, (size_t)w * h,
+                                                 reinterpret_cast<uint32_t *>(c->tmap_dev.p + 128));
             {
                 cudaError_t le = cudaGetLastError();
                 if (le != cudaSuccess) { set_error("k_lum_sobel_tma launch: %s", cudaGetErrorString(le)); return B2TEX_ERR_CUDA; }
@@ -526,17 +470,16 @@ int prepare_images(b2tex_ctx *c, int data_term, bool force)
             B2_CUDA(cudaMemcpyAsync(&timeouts, c->tmap_dev.p + 128, 4, cudaMemcpyDeviceToHost, s));
             B2_CUDA(cudaStreamSynchronize(s));
             if (timeouts) { set_error("k_lum_sobel_tma: %u tile copies never arrived", timeouts); return B2TEX_ERR_CUDA; }
-        } else if (uniform && K <= 65535u && !scalar_sobel) {  // one launch for all views (blockIdx.z = view)
-            int w = c->views_host[0].width, h = c->views_host[0].height;
-            dim3 grid((w + TW2 - 1) / TW2, (h + TH2 - 1) / TH2, K);
-            B2_LAUNCH k_lum_sobel_vec<<<grid, 256, 0, s>>>(c->rgb.p, c->grad.p, w, h, (size_t)w * h, c->rgb.p,
-                                                 c->rgb.p + c->rgb.n);
-        } else {
+        } else {   // the views the TMA kernel declines, of any sizes: one launch, the grid sized for the largest view
+            std::vector<GradView> gv(K);
+            int maxw = 0, maxh = 0;
             for (uint32_t v = 0; v < K; ++v) {
-                int w = c->views_host[v].width, h = c->views_host[v].height;
-                dim3 grid((w + TW - 1) / TW, (h + TH - 1) / TH);
-                B2_LAUNCH k_lum_sobel<<<grid, 256, 0, s>>>(c->rgb.p + 3 * c->img_off[v], c->grad.p + c->img_off[v], w, h);
+                gv[v] = {c->rgb.p + 3 * c->img_off[v], c->grad.p + c->img_off[v], c->views_host[v].width, c->views_host[v].height};
+                maxw = std::max(maxw, gv[v].w); maxh = std::max(maxh, gv[v].h);
             }
+            B2_TRY(gv_dev.upload(gv.data(), K, s));
+            const dim3 grid((maxw + TW - 1) / TW, (maxh + TH - 1) / TH, K);   // K <= 65535 (b2tex_set_views)
+            B2_LAUNCH k_lum_sobel<<<grid, 256, 0, s>>>(gv_dev.p);
         }
         B2_KERNEL_CHECK();
     }

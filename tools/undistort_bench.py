@@ -5,7 +5,7 @@ every view black corners, so that every view gets a validity mask.  Prints one J
                    (3 B gathered + 3 B written per pixel), GB/s and share of the H100 SXM data sheet's 3.35 TB/s;
                    the copy back from the scratch is reported on its own
   flood            the validity flood of prepare_images (k_flood launches plus their host polls, CUDA events) and the
-                   data-cost call around it, per-view rounds (B2TEX_FLOOD_BATCH=1) and batched rounds, alternated
+                   data-cost call around it
   gpu              name and power limit of the card it ran on
 
 The mesh is a small sphere (the C3 cameras and images, not its 1M faces): the data-cost call is then mostly
@@ -73,28 +73,20 @@ def main():
                copy_back=dict(ms=statistics.median(back), bytes=6.0 * px, gbps=6.0 * px / statistics.median(back) / 1e6))
 
     # the undistorted images stay resident: every data-cost call redoes prepare_images with all K views flagged
-    flood = {"per_view": [], "batched": []}
-    call = {"per_view": [], "batched": []}
+    flood, call = [], []
     for rep in range(a.reps + 1):
-        for mode in ("per_view", "batched"):
-            if mode == "per_view":
-                os.environ["B2TEX_FLOOD_BATCH"] = "1"
-            else:
-                os.environ.pop("B2TEX_FLOOD_BATCH", None)
-            c.synchronize()
-            c.profile(True)
-            t0 = time.perf_counter()
-            c.data_costs_run()
-            c.synchronize()
-            t1 = time.perf_counter()
-            rows = c.profile_report()
-            c.profile(False)
-            if rep:
-                flood[mode].append(sum(ms for n, ms, _ in rows if n == "k_flood"))
-                call[mode].append((t1 - t0) * 1e3)
-    os.environ.pop("B2TEX_FLOOD_BATCH", None)
-    res["flood"] = {m: dict(flood_ms=statistics.median(flood[m]), flood_ms_all=flood[m],
-                            data_costs_call_ms=statistics.median(call[m])) for m in flood}
+        c.synchronize()
+        c.profile(True)
+        t0 = time.perf_counter()
+        c.data_costs_run()
+        c.synchronize()
+        t1 = time.perf_counter()
+        rows = c.profile_report()
+        c.profile(False)
+        if rep:
+            flood.append(sum(ms for n, ms, _ in rows if n == "k_flood"))
+            call.append((t1 - t0) * 1e3)
+    res["flood"] = dict(flood_ms=statistics.median(flood), flood_ms_all=flood, data_costs_call_ms=statistics.median(call))
     res["gpu"] = gpu_info()
     c.close()
     line = json.dumps(res)
