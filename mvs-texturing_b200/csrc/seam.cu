@@ -243,12 +243,27 @@ struct Pcg {
     float *x, *r, *t;       // [3][R]
     float4 *p;              // [R] (x,y,z = channels)
     double *partials;       // [2][grid][8]
-    uint32_t *status;       // [0..2] iterations, [3..5] residual bits, [6] loop iterations
+    uint32_t *status;       // [0..2] iterations, [3..5] residual bits, [6] loop iterations,
+                            // [8..13] ns block 0 spent in SpMV / barrier A / update / barrier B / p update / loop-end barrier
     uint32_t max_iters;
     float tol;
+    uint32_t timing;        // diagnostic (B2TEX_SEAM_TIMING): fill status[8..13]
 };
 
-__device__ __forceinline__ void block_reduce6(double v[6], double *smem /* [8][6] */)
+__device__ __forceinline__ unsigned long long pcg_timer_ns()
+{
+#ifdef __CUDA_ARCH__
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+#else
+    return 0ull;
+#endif
+}
+
+// Sum of six doubles over the block in a fixed order: xor butterfly inside every warp, then the warps in order.
+// Only thread 0 ends up with the sums (the other threads go on to the barrier at once).
+__device__ __forceinline__ void block_reduce6(double v[6], double *smem /* [32][6] */)
 {
 #pragma unroll
     for (int k = 0; k < 6; ++k)
@@ -258,6 +273,7 @@ __device__ __forceinline__ void block_reduce6(double v[6], double *smem /* [8][6
     if (lane == 0)
         for (int k = 0; k < 6; ++k) smem[warp * 6 + k] = v[k];
     __syncthreads();
+    if (threadIdx.x != 0) return;
     int nw = blockDim.x >> 5;
     for (int k = 0; k < 6; ++k) {
         double s = 0.0;
@@ -266,17 +282,37 @@ __device__ __forceinline__ void block_reduce6(double v[6], double *smem /* [8][6
     }
 }
 
-// every block sums the per-block partials in the same order -> identical totals everywhere
+// Every block sums the per-block partials in the same order -> identical totals everywhere.  The order is that of
+// block_reduce6 over one partial per thread (nblocks <= blockDim): butterflies over groups of 32 blocks, then the groups
+// in order.  The groups block_reduce6 would add past the last block are +0.0, which leaves a sum that started at +0.0
+// unchanged, so warp 0 alone computes the totals and hands them to the block through shared memory.
 __device__ __forceinline__ void grid_totals(const double *part, int nblocks, double out[6], double *smem)
 {
-    double v[6] = {0, 0, 0, 0, 0, 0};
-    for (int b = threadIdx.x; b < nblocks; b += blockDim.x)
-        for (int k = 0; k < 6; ++k) v[k] += part[(size_t)b * 8 + k];
-    block_reduce6(v, smem);
-    for (int k = 0; k < 6; ++k) out[k] = v[k];
+    if (threadIdx.x < 32) {
+        double s[6] = {0, 0, 0, 0, 0, 0};
+        for (int b0 = 0; b0 < nblocks; b0 += 32) {
+            const int b = b0 + (int)threadIdx.x;
+            double v[6] = {0, 0, 0, 0, 0, 0};
+            if (b < nblocks)
+                for (int k = 0; k < 6; ++k) v[k] += part[(size_t)b * 8 + k];
+#pragma unroll
+            for (int k = 0; k < 6; ++k) {
+                for (int sh = 16; sh; sh >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], sh);
+                s[k] += v[k];
+            }
+        }
+        if (threadIdx.x == 0)
+            for (int k = 0; k < 6; ++k) smem[k] = s[k];
+    }
+    __syncthreads();
+    for (int k = 0; k < 6; ++k) out[k] = smem[k];
 }
 
 constexpr int PCG_THREADS = 1024;  // one fat block per SM: grid.sync() cost grows with the block count
+// Rows / entries per thread in flight.  __launch_bounds__(1024, 1) leaves 64 registers; on C3 (H100 SXM, 400 W)
+// batch 2 / rows 1 spills 48 B and is fastest, batch 4 / rows 2 spills 364 B and is 5 % slower, rows 4 is 20 % slower.
+constexpr int PCG_BATCH = 2;       // SpMV: column words / p gathers per row
+constexpr int PCG_ROWS = 1;        // vector phases: rows per thread
 __global__ void __launch_bounds__(PCG_THREADS, 1) k_pcg(Pcg q)
 {
     cg::grid_group grid = cg::this_grid();
@@ -285,8 +321,13 @@ __global__ void __launch_bounds__(PCG_THREADS, 1) k_pcg(Pcg q)
     const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
     double *partA = q.partials, *partB = q.partials + (size_t)gridDim.x * 8;
     double acc[6], tot[6];
+    const bool prof = q.timing && tid == 0;
+    unsigned long long tprev = prof ? pcg_timer_ns() : 0ull;
+    auto lap = [&](int slot) {
+        if (prof) { const unsigned long long t = pcg_timer_ns(); q.status[8 + slot] += (uint32_t)(t - tprev); tprev = t; }
+    };
 
-    // r = rhs, p = M^-1 r, rhsNorm2 = r.r, absNew = r.p
+    // r = rhs, p = M^-1 r, rhsNorm2 = r.r, absNew = r.p; p.w carries the diagonal for the SpMV and the p update
     for (int k = 0; k < 6; ++k) acc[k] = 0.0;
     for (uint32_t i = tid; i < R; i += nth) {
         float id = q.inv_diag[i];
@@ -299,7 +340,7 @@ __global__ void __launch_bounds__(PCG_THREADS, 1) k_pcg(Pcg q)
             acc[c] += (double)rv[c] * rv[c];
             acc[3 + c] += (double)rv[c] * pv[c];
         }
-        q.p[i] = make_float4(pv[0], pv[1], pv[2], 0.0f);
+        q.p[i] = make_float4(pv[0], pv[1], pv[2], q.diag_val[i]);
     }
     block_reduce6(acc, smem);
     if (threadIdx.x == 0) for (int k = 0; k < 6; ++k) partA[(size_t)blockIdx.x * 8 + k] = acc[k];
@@ -317,31 +358,43 @@ __global__ void __launch_bounds__(PCG_THREADS, 1) k_pcg(Pcg q)
     }
     uint32_t loops = 0;
     grid.sync();  // partA is rewritten below
+    if (prof) tprev = pcg_timer_ns();
     while (active[0] || active[1] || active[2]) {
-        // phase 1: t = A p, p.t.  Two rows per thread in flight: the row loop is a chain of dependent loads
-        // (row extent -> column -> p[column]) and the solve is latency bound, so the second chain is free.
-        // Per row the edges are still added in storage order and the rows of a thread in ascending order: bit-identical.
+        // phase 1: t = A p, p.t.  Two rows per thread; per batch all column words of both rows are loaded first,
+        // then all p gathers, then the products are added: the dependent chain per row is extent -> columns -> p,
+        // once per PCG_BATCH entries instead of once per entry.  Per row the diagonal comes first and the edges
+        // follow in storage order, and the rows of a thread are added in ascending order: bit-identical.
         for (int k = 0; k < 6; ++k) acc[k] = 0.0;
         const float lam2 = 0.1f * 0.1f;
         for (uint32_t i0 = tid; i0 < R; i0 += 2 * nth) {
             const uint32_t i1 = i0 + nth;
             const bool h1 = i1 < R;
+            const uint32_t j1 = h1 ? i1 : i0;
             uint32_t a = q.csr_ptr[i0] + 1, ae = q.csr_ptr[i0 + 1];
-            uint32_t b = h1 ? q.csr_ptr[i1] + 1 : 0u, be = h1 ? q.csr_ptr[i1 + 1] : 0u;
-            const float4 pa = q.p[i0];
-            const float4 pb = h1 ? q.p[i1] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-            const float da = q.diag_val[i0], db = h1 ? q.diag_val[i1] : 0.0f;
-            float a0 = 0.0f + da * pa.x, a1 = 0.0f + da * pa.y, a2 = 0.0f + da * pa.z;  // diagonal first
-            float b0 = 0.0f + db * pb.x, b1 = 0.0f + db * pb.y, b2 = 0.0f + db * pb.z;
+            uint32_t b = q.csr_ptr[j1] + 1, be = h1 ? q.csr_ptr[j1 + 1] : b;
+            const float4 pa = q.p[i0], pb = q.p[j1];
+            float a0 = 0.0f + pa.w * pa.x, a1 = 0.0f + pa.w * pa.y, a2 = 0.0f + pa.w * pa.z;  // diagonal first
+            float b0 = 0.0f + pb.w * pb.x, b1 = 0.0f + pb.w * pb.y, b2 = 0.0f + pb.w * pb.z;
             while (a < ae || b < be) {
-                uint32_t ea = 0, eb = 0;
-                if (a < ae) ea = q.csr_enc[a];
-                if (b < be) eb = q.csr_enc[b];
-                float4 va = make_float4(0.0f, 0.0f, 0.0f, 0.0f), vb = va;
-                if (a < ae) va = q.p[ea & 0x7FFFFFFFu];
-                if (b < be) vb = q.p[eb & 0x7FFFFFFFu];
-                if (a < ae) { const float w = (ea >> 31) ? -1.0f : -lam2; a0 += w * va.x; a1 += w * va.y; a2 += w * va.z; ++a; }
-                if (b < be) { const float w = (eb >> 31) ? -1.0f : -lam2; b0 += w * vb.x; b1 += w * vb.y; b2 += w * vb.z; ++b; }
+                uint32_t ea[PCG_BATCH], eb[PCG_BATCH];
+#pragma unroll
+                for (int k = 0; k < PCG_BATCH; ++k) {
+                    ea[k] = a + k < ae ? q.csr_enc[a + k] : 0u;
+                    eb[k] = b + k < be ? q.csr_enc[b + k] : 0u;
+                }
+                float4 va[PCG_BATCH], vb[PCG_BATCH];
+#pragma unroll
+                for (int k = 0; k < PCG_BATCH; ++k) {
+                    va[k] = a + k < ae ? q.p[ea[k] & 0x7FFFFFFFu] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                    vb[k] = b + k < be ? q.p[eb[k] & 0x7FFFFFFFu] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                }
+#pragma unroll
+                for (int k = 0; k < PCG_BATCH; ++k) {
+                    if (a + k < ae) { const float w = (ea[k] >> 31) ? -1.0f : -lam2; a0 += w * va[k].x; a1 += w * va[k].y; a2 += w * va[k].z; }
+                    if (b + k < be) { const float w = (eb[k] >> 31) ? -1.0f : -lam2; b0 += w * vb[k].x; b1 += w * vb[k].y; b2 += w * vb[k].z; }
+                }
+                a += PCG_BATCH;
+                b += PCG_BATCH;
             }
             q.t[i0] = a0; q.t[(size_t)R + i0] = a1; q.t[2 * (size_t)R + i0] = a2;
             acc[0] += (double)pa.x * a0; acc[1] += (double)pa.y * a1; acc[2] += (double)pa.z * a2;
@@ -352,54 +405,53 @@ __global__ void __launch_bounds__(PCG_THREADS, 1) k_pcg(Pcg q)
         }
         block_reduce6(acc, smem);
         if (threadIdx.x == 0) for (int k = 0; k < 6; ++k) partA[(size_t)blockIdx.x * 8 + k] = acc[k];
+        lap(0);
         grid.sync();
         grid_totals(partA, gridDim.x, tot, smem);
+        lap(1);
         float alpha[3];
-        for (int c = 0; c < 3; ++c) alpha[c] = active[c] ? absNew[c] / (float)tot[c] : 0.0f;
+        bool moved[3];   // channels whose x takes this iteration's step alpha p (applied in phase 3, where p is loaded anyway)
+        for (int c = 0; c < 3; ++c) {
+            alpha[c] = active[c] ? absNew[c] / (float)tot[c] : 0.0f;
+            moved[c] = active[c];
+        }
 
-        // phase 2: x += a p, r -= a t, |r|^2, r.z (two rows per thread in flight, loads first)
+        // phase 2: r -= a t, |r|^2, r.z (PCG_ROWS rows per thread in flight, loads first, rows added in ascending order)
         for (int k = 0; k < 6; ++k) acc[k] = 0.0;
-        for (uint32_t i0 = tid; i0 < R; i0 += 2 * nth) {
-            const uint32_t i1 = i0 + nth;
-            const bool h1 = i1 < R;
-            const uint32_t j1 = h1 ? i1 : i0;
-            const float4 pa = q.p[i0], pb = q.p[j1];
-            const float ida = q.inv_diag[i0], idb = q.inv_diag[j1];
-            float xa[3], ra[3], ta[3], xb[3], rb[3], tb[3];
+        for (uint32_t i = tid; i < R; i += PCG_ROWS * nth) {
+            float id[PCG_ROWS], rr[PCG_ROWS][3], tt[PCG_ROWS][3];
 #pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const size_t oa = (size_t)c * R + i0, ob = (size_t)c * R + j1;
-                xa[c] = q.x[oa]; ra[c] = q.r[oa]; ta[c] = q.t[oa];
-                xb[c] = q.x[ob]; rb[c] = q.r[ob]; tb[c] = q.t[ob];
-            }
-            const float pva[3] = {pa.x, pa.y, pa.z}, pvb[3] = {pb.x, pb.y, pb.z};
+            for (int u = 0; u < PCG_ROWS; ++u) {
+                const uint32_t j = i + u * nth;
+                id[u] = 0.0f;
 #pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                if (!active[c]) continue;
-                const size_t oa = (size_t)c * R + i0;
-                q.x[oa] = xa[c] + alpha[c] * pva[c];
-                const float rv = ra[c] - alpha[c] * ta[c];
-                q.r[oa] = rv;
-                acc[c] += (double)rv * rv;
-                acc[3 + c] += (double)rv * (ida * rv);
+                for (int c = 0; c < 3; ++c) { rr[u][c] = 0.0f; tt[u][c] = 0.0f; }
+                if (j >= R) continue;
+                id[u] = q.inv_diag[j];
+#pragma unroll
+                for (int c = 0; c < 3; ++c)
+                    if (active[c]) { rr[u][c] = q.r[(size_t)c * R + j]; tt[u][c] = q.t[(size_t)c * R + j]; }
             }
-            if (h1) {
+#pragma unroll
+            for (int u = 0; u < PCG_ROWS; ++u) {
+                const uint32_t j = i + u * nth;
+                if (j >= R) continue;
 #pragma unroll
                 for (int c = 0; c < 3; ++c) {
                     if (!active[c]) continue;
-                    const size_t ob = (size_t)c * R + i1;
-                    q.x[ob] = xb[c] + alpha[c] * pvb[c];
-                    const float rv = rb[c] - alpha[c] * tb[c];
-                    q.r[ob] = rv;
+                    const float rv = rr[u][c] - alpha[c] * tt[u][c];
+                    q.r[(size_t)c * R + j] = rv;
                     acc[c] += (double)rv * rv;
-                    acc[3 + c] += (double)rv * (idb * rv);
+                    acc[3 + c] += (double)rv * (id[u] * rv);
                 }
             }
         }
         block_reduce6(acc, smem);
         if (threadIdx.x == 0) for (int k = 0; k < 6; ++k) partB[(size_t)blockIdx.x * 8 + k] = acc[k];
+        lap(2);
         grid.sync();
         grid_totals(partB, gridDim.x, tot, smem);
+        lap(3);
         float beta[3] = {0.0f, 0.0f, 0.0f};
         bool upd[3];
         for (int c = 0; c < 3; ++c) {
@@ -413,25 +465,46 @@ __global__ void __launch_bounds__(PCG_THREADS, 1) k_pcg(Pcg q)
             upd[c] = true;
             if (++iters[c] >= q.max_iters) active[c] = false;  // while (i < maxIters)
         }
-        // phase 3: p = z + beta p (two rows per thread in flight)
-        if (upd[0] || upd[1] || upd[2]) {
-            for (uint32_t i0 = tid; i0 < R; i0 += 2 * nth) {
-                const uint32_t i1 = i0 + nth;
-                const bool h1 = i1 < R;
-                const uint32_t j1 = h1 ? i1 : i0;
-                float4 pa = q.p[i0], pb = q.p[j1];
-                const float ida = q.inv_diag[i0], idb = q.inv_diag[j1];
-                const float ra0 = q.r[i0], ra1 = q.r[(size_t)R + i0], ra2 = q.r[2 * (size_t)R + i0];
-                const float rb0 = q.r[j1], rb1 = q.r[(size_t)R + j1], rb2 = q.r[2 * (size_t)R + j1];
-                if (upd[0]) { pa.x = ida * ra0 + beta[0] * pa.x; pb.x = idb * rb0 + beta[0] * pb.x; }
-                if (upd[1]) { pa.y = ida * ra1 + beta[1] * pa.y; pb.y = idb * rb1 + beta[1] * pb.y; }
-                if (upd[2]) { pa.z = ida * ra2 + beta[2] * pa.z; pb.z = idb * rb2 + beta[2] * pb.z; }
-                q.p[i0] = pa;
-                if (h1) q.p[i1] = pb;
+        // phase 3: x += a p with the p of this iteration, then p = z + beta p (PCG_ROWS rows per thread in flight).
+        // Runs in every iteration: some channel was active in phase 2, or the loop would have ended.
+        const bool pu = upd[0] || upd[1] || upd[2];
+        for (uint32_t i = tid; i < R; i += PCG_ROWS * nth) {
+            float4 pv[PCG_ROWS];
+            float xx[PCG_ROWS][3], rr[PCG_ROWS][3];
+#pragma unroll
+            for (int u = 0; u < PCG_ROWS; ++u) {
+                const uint32_t j = i + u * nth;
+                pv[u] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+#pragma unroll
+                for (int c = 0; c < 3; ++c) { xx[u][c] = 0.0f; rr[u][c] = 0.0f; }
+                if (j >= R) continue;
+                pv[u] = q.p[j];
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    if (moved[c]) xx[u][c] = q.x[(size_t)c * R + j];
+                    if (upd[c]) rr[u][c] = q.r[(size_t)c * R + j];
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < PCG_ROWS; ++u) {
+                const uint32_t j = i + u * nth;
+                if (j >= R) continue;
+                if (moved[0]) q.x[j] = xx[u][0] + alpha[0] * pv[u].x;
+                if (moved[1]) q.x[(size_t)R + j] = xx[u][1] + alpha[1] * pv[u].y;
+                if (moved[2]) q.x[2 * (size_t)R + j] = xx[u][2] + alpha[2] * pv[u].z;
+                if (!pu) continue;
+                const float d = pv[u].w;
+                const float id = d != 0.0f ? 1.0f / d : 1.0f;   // = inv_diag (k_matrix): same expression, same bits
+                if (upd[0]) pv[u].x = id * rr[u][0] + beta[0] * pv[u].x;
+                if (upd[1]) pv[u].y = id * rr[u][1] + beta[1] * pv[u].y;
+                if (upd[2]) pv[u].z = id * rr[u][2] + beta[2] * pv[u].z;
+                q.p[j] = pv[u];
             }
         }
+        lap(4);
         ++loops;
         grid.sync();
+        lap(5);
     }
     // x -= mean(x)  (:277)
     for (int k = 0; k < 6; ++k) acc[k] = 0.0;
@@ -561,9 +634,12 @@ int seam_run(b2tex_ctx *c, b2tex_seam_info *info, bool solve)
         int grid = c->num_sms * per_sm;
         int need = (int)((R + PCG_THREADS - 1) / PCG_THREADS);
         if (grid > need) grid = std::max(1, need);
+        grid = std::min(grid, PCG_THREADS);   // grid_totals: at most one block partial per thread
         B2_TRY(c->seam_partials.alloc(2 * (size_t)grid * 8));
         Pcg q{R, c->csr_ptr.p, c->csr_enc.p, c->seam_dval.p, c->seam_diag.p, c->seam_rhs.p, c->seam_x.p,
               c->seam_r.p, c->seam_t.p, c->seam_p.p, c->seam_partials.p, c->seam_status.p, 1000u, 0.0001f};
+        static const bool seam_timing = getenv("B2TEX_SEAM_TIMING") != nullptr;
+        q.timing = seam_timing ? 1u : 0u;
         void *args[] = {&q};
         cudaEvent_t e0, e1;
         B2_CUDA(cudaEventCreate(&e0));
@@ -572,13 +648,17 @@ int seam_run(b2tex_ctx *c, b2tex_seam_info *info, bool solve)
         count_launch();
         B2_CUDA(cudaLaunchCooperativeKernel((void *)k_pcg, dim3(grid), dim3(PCG_THREADS), args, 0, s));
         B2_CUDA(cudaEventRecord(e1, s));
-        uint32_t st[8];
+        uint32_t st[16];
         B2_CUDA(cudaMemcpyAsync(st, c->seam_status.p, sizeof(st), cudaMemcpyDeviceToHost, s));
         B2_CUDA(cudaStreamSynchronize(s));
         float ms = 0.0f;
         cudaEventElapsedTime(&ms, e0, e1);
         cudaEventDestroy(e0);
         cudaEventDestroy(e1);
+        if (seam_timing)
+            fprintf(stderr, "k_pcg: %u iterations, grid %d, %.3f ms, block 0 [us]: spmv %.0f barrier_a %.0f update %.0f barrier_b %.0f "
+                    "p %.0f loop_barrier %.0f\n", st[6], grid, ms, st[8] / 1e3, st[9] / 1e3, st[10] / 1e3, st[11] / 1e3, st[12] / 1e3,
+                    st[13] / 1e3);
         for (int ch = 0; ch < 3; ++ch) {
             info->iterations[ch] = st[ch];
             memcpy(&info->residual[ch], &st[3 + ch], 4);

@@ -5,7 +5,8 @@
                              [--out DIR]
 
 Both trees must have been built (libb2tex.so next to their package).  Per run it prints ms_per_step,
-stage_ms.data_costs, the data-cost kernel groups bench.py reports, verify.crc_data_costs / crc_labels and the
+stage_ms.data_costs and .seam_leveling, the k_pcg time (its own events), the data-cost kernel groups bench.py reports,
+verify.crc_data_costs / crc_labels and the
 verify flags; every run also writes `--dump-outputs` to DIR/<label>_<i>/, and the outputs of all runs are compared
 byte for byte (by sha256; the dumps are removed afterwards unless --keep-dumps).  Then one profiling pass per tree
 (same workload, profiler on) lists EVERY kernel group of the data-cost stage, including those below bench.py's top ten.  The GPU name and power limit are read in the same invocation.
@@ -110,8 +111,11 @@ def main():
                 json.dump(res, f)
             v = res.get("verify") or {}
             kern = {k["name"]: round(k["ms_per_step"], 3) for k in res["kernels"] if k["name"].startswith(DC_PREFIXES)}
+            pcg = next((k for k in res["kernels"] if k["name"] in ("k_pcg", "k_pcg_mg")), None)
             row = {"build": label, "run": i, "ms_per_step": round(res["ms_per_step"], 2),
                    "data_costs_ms": round(res["stage_ms"].get("data_costs", float("nan")), 2), "dc_kernels_top10": kern,
+                   "seam_leveling_ms": round(res["stage_ms"].get("seam_leveling", float("nan")), 2),
+                   "k_pcg_ms": round(pcg["ms_per_step"], 3) if pcg else None,
                    "verify_ok": v.get("ok"), "data_costs_bit_exact": v.get("data_costs_bit_exact"),
                    "labels_bit_exact": v.get("labels_bit_exact"), "mrf_energy_identical": v.get("mrf_energy_identical"),
                    "crc_data_costs": v.get("crc_data_costs"), "crc_labels": v.get("crc_labels"),
@@ -125,8 +129,11 @@ def main():
     for label, rs in rows.items():
         ms = [r["ms_per_step"] for r in rs]
         dc = [r["data_costs_ms"] for r in rs]
+        sl = [r["seam_leveling_ms"] for r in rs]
+        pcg = [r["k_pcg_ms"] for r in rs if r["k_pcg_ms"] is not None]
         summary[label] = {"ms_per_step": ms, "median": sorted(ms)[len(ms) // 2], "spread": max(ms) - min(ms),
-                          "data_costs_ms": dc, "data_costs_median": sorted(dc)[len(dc) // 2]}
+                          "data_costs_ms": dc, "data_costs_median": sorted(dc)[len(dc) // 2],
+                          "seam_leveling_ms": sl, "k_pcg_ms": pcg, "k_pcg_median": sorted(pcg)[len(pcg) // 2] if pcg else None}
     summary["gain_ms"] = summary["base"]["median"] - summary["new"]["median"]
     summary["gain_over_3x_spread"] = summary["gain_ms"] > 3 * max(summary["base"]["spread"], summary["new"]["spread"])
     all_rows = rows["base"] + rows["new"]
