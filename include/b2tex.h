@@ -112,6 +112,15 @@ typedef struct {
     float dist[2];   /* dist[0] == 0: no distortion; dist[1] != 0: Bundler k2 k4 model; else VisualSFM with k = dist[0] */
 } b2tex_distortion;
 
+/* sizes of the mesh graph b2tex_build_mesh_graph derives */
+typedef struct {
+    uint32_t num_adjacency;          /* adj_ptr[F]: directed face-adjacency entries */
+    uint32_t num_vertex_faces;       /* vf_ptr[Vn] */
+    uint32_t num_vertex_neighbours;  /* vv_ptr[Vn] */
+    uint32_t max_face_degree;        /* longest adjacency row */
+    uint32_t num_non_manifold_edges; /* undirected edges shared by more than two faces */
+} b2tex_graph_info;
+
 typedef struct b2tex_ctx b2tex_ctx;
 
 /* ---- lifetime ---- */
@@ -134,6 +143,19 @@ int b2tex_set_views(b2tex_ctx *ctx, const b2tex_view *views, uint32_t num_views)
 int b2tex_set_adjacency(b2tex_ctx *ctx, const uint32_t *adj_ptr, const uint32_t *adj_idx);
 int b2tex_set_vertex_rings(b2tex_ctx *ctx, const uint32_t *vf_ptr, const uint32_t *vf_idx,
                            const uint32_t *vv_ptr, const uint32_t *vv_idx);
+/* Derives the face adjacency (build_adjacency_graph.cpp:16-53) and the vertex rings from the mesh set by b2tex_set_mesh,
+ * on the device; afterwards the context is as if b2tex_set_adjacency and b2tex_set_vertex_rings had been called with the
+ * arrays scene.face_adjacency / scene.vertex_rings give: adjacency rows hold the lower neighbours ascending, then the
+ * higher ones by the slot of the shared edge and ascending, each face once; vf rows the incident faces ascending (a face
+ * with a repeated vertex twice); vv rows the distinct u of the directed edges (v, u) ascending.  B2TEX_ERR_ARG without a
+ * mesh or with a face index >= num_verts (the first such face is named); B2TEX_ERR_LIMITS when a count does not fit the
+ * 32-bit offsets.  A failed build leaves the context without a graph.  info may be NULL. */
+int b2tex_build_mesh_graph(b2tex_ctx *ctx, b2tex_graph_info *info);
+/* the resident graph (derived or uploaded); arrays sized from b2tex_graph_info: adj_ptr[F+1], adj_idx[num_adjacency],
+ * vf_ptr[Vn+1], vf_idx[num_vertex_faces], vv_ptr[Vn+1], vv_idx[num_vertex_neighbours]; any pointer may be NULL;
+ * B2TEX_ERR_ARG when a requested part is not resident */
+int b2tex_mesh_graph_download(b2tex_ctx *ctx, uint32_t *adj_ptr, uint32_t *adj_idx, uint32_t *vf_ptr, uint32_t *vf_idx,
+                              uint32_t *vv_ptr, uint32_t *vv_idx);
 int b2tex_set_data_costs(b2tex_ctx *ctx, const uint64_t *face_ptr, const uint16_t *view,
                          const float *cost);
 int b2tex_set_labels(b2tex_ctx *ctx, const uint32_t *labels);
@@ -261,7 +283,9 @@ int b2tex_view_selection(uint32_t num_faces, const uint32_t *adj_ptr, const uint
                          const b2tex_mrf_params *params_or_null, uint32_t *labels_out,
                          b2tex_mrf_info *info);
 /* tex::global_seam_leveling up to the per-(vertex,label) adjust values (:283-289):
- * row_ptr_out[Vn+1] caller allocated; row_label/x (R and R*3, centred) malloc'ed by the library. */
+ * row_ptr_out[Vn+1] caller allocated; row_label/x (R and R*3, centred) malloc'ed by the library.
+ * vf_ptr, vf_idx, vv_ptr and vv_idx all NULL: the rings are derived from the mesh on the device (b2tex_build_mesh_graph);
+ * some NULL and some not: B2TEX_ERR_ARG. */
 int b2tex_global_seam_leveling(const float *verts, uint32_t num_verts, const uint32_t *faces,
                                uint32_t num_faces, const uint32_t *vf_ptr, const uint32_t *vf_idx,
                                const uint32_t *vv_ptr, const uint32_t *vv_idx,
@@ -272,7 +296,9 @@ int b2tex_global_seam_leveling(const float *verts, uint32_t num_verts, const uin
 /* The three stages back to back on one upload -- what texrecon does between texrecon.cpp:100 and :171
  * when it writes no intermediate results (--no_intermediate_results, arguments.cpp:88-89): the mesh and
  * the images cross PCIe once, DataCosts stay on the device, only labels[F] and the per-(vertex,label)
- * adjust values come back.  Optional outputs may be NULL.  row_label/x are malloc'ed (b2tex_free). */
+ * adjust values come back.  Optional outputs may be NULL.  row_label/x are malloc'ed (b2tex_free).
+ * The six topology arrays (adj_ptr .. vv_idx) all NULL: the graph is derived from the mesh on the device
+ * (b2tex_build_mesh_graph); some NULL and some not: B2TEX_ERR_ARG. */
 int b2tex_texture_hot_path(const float *verts, uint32_t num_verts, const uint32_t *faces,
                            const float *face_normals, uint32_t num_faces, const b2tex_view *views,
                            uint32_t num_views, const uint32_t *adj_ptr, const uint32_t *adj_idx,
@@ -284,7 +310,9 @@ int b2tex_texture_hot_path(const float *verts, uint32_t num_verts, const uint32_
 
 /* Everything texrecon does between texrecon.cpp:160 and :189 on one upload: texture patches for the seen faces,
  * global seam leveling (do_global; else the zero-offset validity pass of :174-183), local seam leveling (do_local).
- * Outputs are malloc'ed (b2tex_free) and laid out as b2tex_texture_patches_download describes; info structs may be NULL. */
+ * Outputs are malloc'ed (b2tex_free) and laid out as b2tex_texture_patches_download describes; info structs may be NULL.
+ * The six topology arrays (adj_ptr .. vv_idx) all NULL: the graph is derived from the mesh on the device
+ * (b2tex_build_mesh_graph); some NULL and some not: B2TEX_ERR_ARG. */
 int b2tex_seam_leveling_patches(const float *verts, uint32_t num_verts, const uint32_t *faces, uint32_t num_faces,
                                 const uint32_t *adj_ptr, const uint32_t *adj_idx, const uint32_t *vf_ptr,
                                 const uint32_t *vf_idx, const uint32_t *vv_ptr, const uint32_t *vv_idx,

@@ -124,13 +124,14 @@ int b2tex_set_mesh(b2tex_ctx *c, const float *verts, uint32_t nv, const uint32_t
 {
     B2_CUDA(cudaSetDevice(c->device));
     if (!verts || !faces || !normals) { set_error("set_mesh: null pointer"); return B2TEX_ERR_ARG; }
+    c->have_mesh = false;
     c->Vn = nv; c->F = nf; c->face_begin = 0; c->face_end = nf;
     B2_TRY(c->verts.upload(verts, 3 * (size_t)nv, c->stream));
     B2_TRY(c->faces.upload(faces, 3 * (size_t)nf, c->stream));
     B2_TRY(c->normals.upload(normals, 3 * (size_t)nf, c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
     c->bvh_built = false; c->have_costs = false; c->have_labels = false; c->have_adj = false;
-    c->have_rings = false; c->mrf_ready = false; c->have_seam = false;
+    c->have_rings = false; c->mrf_ready = false; c->have_seam = false; c->have_mesh = true;
     return B2TEX_OK;
 }
 
@@ -212,6 +213,32 @@ int b2tex_set_vertex_rings(b2tex_ctx *c, const uint32_t *vf_ptr, const uint32_t 
     B2_TRY(c->vv_idx.upload(vv_idx, vv_ptr[c->Vn], c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
     c->have_rings = true;
+    return B2TEX_OK;
+}
+
+int b2tex_build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info)
+{
+    B2_CUDA(cudaSetDevice(c->device));
+    return build_mesh_graph(c, info);
+}
+
+int b2tex_mesh_graph_download(b2tex_ctx *c, uint32_t *adj_ptr, uint32_t *adj_idx, uint32_t *vf_ptr, uint32_t *vf_idx,
+                              uint32_t *vv_ptr, uint32_t *vv_idx)
+{
+    B2_CUDA(cudaSetDevice(c->device));
+    if (!c->have_adj && !c->have_rings) { set_error("mesh_graph_download: no graph is resident"); return B2TEX_ERR_ARG; }
+    if ((adj_ptr || adj_idx) && !c->have_adj) { set_error("mesh_graph_download: no face adjacency is resident"); return B2TEX_ERR_ARG; }
+    if ((vf_ptr || vf_idx || vv_ptr || vv_idx) && !c->have_rings) {
+        set_error("mesh_graph_download: no vertex rings are resident");
+        return B2TEX_ERR_ARG;
+    }
+    if (adj_ptr) B2_TRY(c->adj_ptr.download(adj_ptr, (size_t)c->F + 1, c->stream));
+    if (adj_idx) B2_TRY(c->adj_idx.download(adj_idx, c->adj_idx.n, c->stream));
+    if (vf_ptr) B2_TRY(c->vf_ptr.download(vf_ptr, (size_t)c->Vn + 1, c->stream));
+    if (vf_idx) B2_TRY(c->vf_idx.download(vf_idx, c->vf_idx.n, c->stream));
+    if (vv_ptr) B2_TRY(c->vv_ptr.download(vv_ptr, (size_t)c->Vn + 1, c->stream));
+    if (vv_idx) B2_TRY(c->vv_idx.download(vv_idx, c->vv_idx.n, c->stream));
+    B2_CUDA(cudaStreamSynchronize(c->stream));
     return B2TEX_OK;
 }
 
@@ -482,6 +509,7 @@ static int acquire_ctx(b2tex_ctx **out)
                 b2tex_ctx *c = g_pool[i];
                 g_pool.erase(g_pool.begin() + (long)i);
                 c->have_costs = c->have_labels = c->have_adj = c->have_rings = c->mrf_ready = c->have_seam = false;
+                c->have_mesh = false;
                 c->images_prepared = false; c->prepared_data_term = -1; c->bvh_built = false;
                 c->Vn = c->F = c->K = 0; c->face_begin = c->face_end = 0; c->nnz = 0; c->R = 0;
                 *out = c;
@@ -506,6 +534,17 @@ void b2tex_release_cached_contexts(void)
     std::vector<b2tex_ctx *> v;
     { std::lock_guard<std::mutex> lk(g_pool_mu); v.swap(g_pool); }
     for (b2tex_ctx *c : v) b2tex_destroy(c);
+}
+
+// topology arrays of a one-shot call: 0 = all given, 1 = all NULL (derived on the device), -1 = a mix (error set)
+static int topology_nulls(const char *fn, std::initializer_list<const uint32_t *> arrays)
+{
+    size_t nulls = 0;
+    for (const uint32_t *a : arrays) nulls += a == nullptr;
+    if (nulls == 0) return 0;
+    if (nulls == arrays.size()) return 1;
+    set_error("%s: the topology arrays must be all given or all NULL (%zu of %zu are NULL)", fn, nulls, arrays.size());
+    return -1;
 }
 
 static int dc_oneshot(const float *verts, uint32_t nv, const uint32_t *faces, const float *normals, uint32_t nf,
@@ -610,12 +649,14 @@ int b2tex_global_seam_leveling(const float *verts, uint32_t nv, const uint32_t *
                                const uint32_t *vv_idx, const uint32_t *labels, const b2tex_view *views, uint32_t K,
                                uint32_t *row_ptr_out, uint32_t **row_label_out, float **x_out, b2tex_seam_info *info)
 {
+    const int derive = topology_nulls("global_seam_leveling", {vf_ptr, vf_idx, vv_ptr, vv_idx});
+    if (derive < 0) return B2TEX_ERR_ARG;
     b2tex_ctx *c = nullptr;
     B2_TRY(acquire_ctx(&c));
     std::vector<float> dummy_normals(3 * (size_t)nf, 0.0f);
     int rc = b2tex_set_mesh(c, verts, nv, faces, dummy_normals.data(), nf);
     if (rc == B2TEX_OK) rc = b2tex_set_views(c, views, K);
-    if (rc == B2TEX_OK) rc = b2tex_set_vertex_rings(c, vf_ptr, vf_idx, vv_ptr, vv_idx);
+    if (rc == B2TEX_OK) rc = derive ? b2tex_build_mesh_graph(c, nullptr) : b2tex_set_vertex_rings(c, vf_ptr, vf_idx, vv_ptr, vv_idx);
     if (rc == B2TEX_OK) rc = b2tex_set_labels(c, labels);
     if (rc == B2TEX_OK) rc = b2tex_seam_run(c, info);
     if (rc == B2TEX_OK) {
@@ -634,6 +675,8 @@ int b2tex_seam_leveling_patches(const float *verts, uint32_t nv, const uint32_t 
                                 uint8_t **validity_out, b2tex_patch_info *pi, b2tex_seam_info *si, b2tex_local_seam_info *li)
 {
     if (K > 65535u) { set_error("Exeeded maximal number of views"); return B2TEX_ERR_LIMITS; }
+    const int derive = topology_nulls("seam_leveling_patches", {adj_ptr, adj_idx, vf_ptr, vf_idx, vv_ptr, vv_idx});
+    if (derive < 0) return B2TEX_ERR_ARG;
     b2tex_ctx *c = nullptr;
     B2_TRY(acquire_ctx(&c));
     b2tex_patch_info pl; b2tex_seam_info sl; b2tex_local_seam_info ll;
@@ -644,8 +687,9 @@ int b2tex_seam_leveling_patches(const float *verts, uint32_t nv, const uint32_t 
     std::vector<float> dummy_normals(3 * (size_t)nf, 0.0f);
     int rc = b2tex_set_mesh(c, verts, nv, faces, dummy_normals.data(), nf);
     if (rc == B2TEX_OK) rc = b2tex_set_views(c, views, K);
-    if (rc == B2TEX_OK) rc = b2tex_set_adjacency(c, adj_ptr, adj_idx);
-    if (rc == B2TEX_OK) rc = b2tex_set_vertex_rings(c, vf_ptr, vf_idx, vv_ptr, vv_idx);
+    if (rc == B2TEX_OK && derive) rc = b2tex_build_mesh_graph(c, nullptr);
+    if (rc == B2TEX_OK && !derive) rc = b2tex_set_adjacency(c, adj_ptr, adj_idx);
+    if (rc == B2TEX_OK && !derive) rc = b2tex_set_vertex_rings(c, vf_ptr, vf_idx, vv_ptr, vv_idx);
     if (rc == B2TEX_OK) rc = b2tex_set_labels(c, labels);
     if (rc == B2TEX_OK && do_global) rc = b2tex_seam_run(c, si);
     if (rc == B2TEX_OK) rc = b2tex_texture_patches_run(c, do_global ? 1 : 0, pi);
@@ -675,6 +719,8 @@ int b2tex_texture_hot_path(const float *verts, uint32_t nv, const uint32_t *face
                            b2tex_dc_info *dci, b2tex_mrf_info *mi, b2tex_seam_info *si)
 {
     if (K > 65535u) { set_error("Exeeded maximal number of views"); return B2TEX_ERR_LIMITS; }
+    const int derive = topology_nulls("texture_hot_path", {adj_ptr, adj_idx, vf_ptr, vf_idx, vv_ptr, vv_idx});
+    if (derive < 0) return B2TEX_ERR_ARG;
     b2tex_ctx *c = nullptr;
     B2_TRY(acquire_ctx(&c));
     b2tex_dc_info dc_local; b2tex_mrf_info mrf_local; b2tex_seam_info seam_local;
@@ -687,8 +733,9 @@ int b2tex_texture_hot_path(const float *verts, uint32_t nv, const uint32_t *face
     c->defer_image_sync = true;
     if (rc == B2TEX_OK) rc = b2tex_set_views(c, views, K);
     c->defer_image_sync = false;
-    if (rc == B2TEX_OK) rc = b2tex_set_adjacency(c, adj_ptr, adj_idx);
-    if (rc == B2TEX_OK) rc = b2tex_set_vertex_rings(c, vf_ptr, vf_idx, vv_ptr, vv_idx);
+    if (rc == B2TEX_OK && derive) rc = b2tex_build_mesh_graph(c, nullptr);   // runs while the images cross PCIe
+    if (rc == B2TEX_OK && !derive) rc = b2tex_set_adjacency(c, adj_ptr, adj_idx);
+    if (rc == B2TEX_OK && !derive) rc = b2tex_set_vertex_rings(c, vf_ptr, vf_idx, vv_ptr, vv_idx);
     if (rc == B2TEX_OK) rc = b2tex_data_costs_run(c, st, dci);
     if (c->images_in_flight) { cudaStreamSynchronize(c->copy_stream); c->images_in_flight = false; }   // also on the error paths
     if (rc == B2TEX_OK) rc = b2tex_view_selection_run(c, mp, mi, nullptr);

@@ -156,6 +156,7 @@ struct b2tex_ctx {
     uint32_t face_begin = 0, face_end = 0;
     b2::DevBuf<float> verts, normals;
     b2::DevBuf<uint32_t> faces;
+    bool have_mesh = false;   // set_mesh has run (view selection alone sets F without a mesh)
 
     // views
     uint32_t K = 0;
@@ -226,6 +227,10 @@ struct b2tex_ctx {
     // seam
     b2::DevBuf<uint32_t> vf_ptr, vf_idx, vv_ptr, vv_idx;
     bool have_rings = false;
+    // scratch of the mesh-graph build (graph.cu): sort keys [6F] x 2, values [3F] x 2, counts / run heads [6F], scalars
+    b2::DevBuf<uint64_t> g_key[2];
+    b2::DevBuf<uint32_t> g_val[2], g_cnt;
+    b2::DevBuf<unsigned long long> g_scal;
     b2::DevBuf<uint32_t> row_ptr, row_label, arow_ptr, arow_rows;
     b2::DevBuf<float> arow_b;
     b2::DevBuf<uint32_t> csr_ptr, csr_col, csr_enc;
@@ -302,6 +307,7 @@ int patches_download(b2tex_ctx *c, int32_t *desc, uint32_t *faces, float *texcoo
                      uint8_t *blending);
 void patches_free(b2tex_ctx *c);
 int local_seam_run(b2tex_ctx *c, b2tex_local_seam_info *info);
+int build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info);
 int cub_exclusive_sum_u64(b2tex_ctx *c, const uint64_t *in, uint64_t *out, size_t n);
 int cub_exclusive_sum_u32(b2tex_ctx *c, const uint32_t *in, uint32_t *out, size_t n);
 }  // namespace b2
