@@ -10,6 +10,7 @@
  *   tex::view_selection         libs/tex/texturing.h:79-80  -> b2tex_view_selection
  *   tex::global_seam_leveling   libs/tex/texturing.h:97-101 -> b2tex_global_seam_leveling
  *   (build_adjacency_graph      libs/tex/texturing.h:59-61  input of view_selection, passed as CSR)
+ *   tex::prepare_mesh           libs/tex/texturing.h:46     -> b2tex_prepare_mesh (resident API)
  *
  * Plain pointers and sizes only; host buffers are owned by the caller, device memory by the
  * library.  Every function returns 0 on success and a non-zero status otherwise;
@@ -121,6 +122,15 @@ typedef struct {
     uint32_t num_non_manifold_edges; /* undirected edges shared by more than two faces */
 } b2tex_graph_info;
 
+/* what b2tex_prepare_mesh did */
+typedef struct {
+    uint32_t num_faces_in;       /* faces passed in */
+    uint32_t num_faces;          /* faces kept (F of the context afterwards) */
+    uint32_t num_redundant;      /* "Removed N redundant faces." (prepare_mesh.cpp:60) */
+    uint32_t num_zero_normals;   /* kept faces whose normal is 0 */
+    b2tex_graph_info graph;      /* what b2tex_build_mesh_graph reports for the kept faces */
+} b2tex_mesh_prep_info;
+
 typedef struct b2tex_ctx b2tex_ctx;
 
 /* ---- lifetime ---- */
@@ -156,6 +166,21 @@ int b2tex_build_mesh_graph(b2tex_ctx *ctx, b2tex_graph_info *info);
  * B2TEX_ERR_ARG when a requested part is not resident */
 int b2tex_mesh_graph_download(b2tex_ctx *ctx, uint32_t *adj_ptr, uint32_t *adj_idx, uint32_t *vf_ptr, uint32_t *vf_idx,
                               uint32_t *vv_ptr, uint32_t *vv_idx);
+/* tex::prepare_mesh (prepare_mesh.cpp:14-70) on the raw mesh, as texrecon loads it: face i is dropped when a face j > i has
+ * all its vertices among those of i (exact duplicates in any order keep the highest id; a proper triangle also goes when a
+ * later degenerate face such as (a, a, b) uses only its vertices), the kept faces stay in their order, the vertices are
+ * untouched.  Then the face normals of the kept faces (normalised cross(b - a, c - a), 0 when its length is 0), the mesh
+ * graph (b2tex_build_mesh_graph) and angle-weighted vertex normals.  Afterwards the context is exactly as after
+ * b2tex_set_mesh(verts, kept faces, their normals) + b2tex_build_mesh_graph, with the vertex normals resident; results of
+ * earlier stages are discarded.  B2TEX_ERR_ARG for NULL pointers, num_faces == 0 or a face index >= num_verts (the first
+ * such face is named); B2TEX_ERR_LIMITS when a count does not fit the 32-bit offsets.  A failure leaves no mesh.  info may
+ * be NULL. */
+int b2tex_prepare_mesh(b2tex_ctx *ctx, const float *verts, uint32_t num_verts, const uint32_t *faces,
+                       uint32_t num_faces, b2tex_mesh_prep_info *info);
+/* faces[F'][3], face_normals[F'][3], vertex_normals[Vn][3], kept_face_ids[F'] (old id of each kept face); any may be NULL.
+ * B2TEX_ERR_ARG unless the last b2tex_prepare_mesh / b2tex_set_mesh on this context was a successful prepare. */
+int b2tex_prepared_mesh_download(b2tex_ctx *ctx, uint32_t *faces, float *face_normals, float *vertex_normals,
+                                 uint32_t *kept_face_ids);
 int b2tex_set_data_costs(b2tex_ctx *ctx, const uint64_t *face_ptr, const uint16_t *view,
                          const float *cost);
 int b2tex_set_labels(b2tex_ctx *ctx, const uint32_t *labels);

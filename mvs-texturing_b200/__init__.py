@@ -33,7 +33,7 @@ EXPORTS = [
     "b2tex_seam_mg_solve", "b2tex_mrf_mg_export", "b2tex_mrf_mg_import", "b2tex_peer_block", "b2tex_peer_attach",
     "b2tex_calculate_data_costs", "b2tex_calculate_data_costs_into", "b2tex_postprocess_face_infos", "b2tex_view_selection",
     "b2tex_global_seam_leveling", "b2tex_texture_hot_path", "b2tex_seam_leveling_patches", "b2tex_release_cached_contexts",
-    "b2tex_build_mesh_graph", "b2tex_mesh_graph_download",
+    "b2tex_build_mesh_graph", "b2tex_mesh_graph_download", "b2tex_prepare_mesh", "b2tex_prepared_mesh_download",
 ]
 
 
@@ -86,6 +86,11 @@ class B2SeamInfo(C.Structure):
 class B2GraphInfo(C.Structure):
     _fields_ = [("num_adjacency", C.c_uint32), ("num_vertex_faces", C.c_uint32), ("num_vertex_neighbours", C.c_uint32),
                 ("max_face_degree", C.c_uint32), ("num_non_manifold_edges", C.c_uint32)]
+
+
+class B2MeshPrepInfo(C.Structure):
+    _fields_ = [("num_faces_in", C.c_uint32), ("num_faces", C.c_uint32), ("num_redundant", C.c_uint32),
+                ("num_zero_normals", C.c_uint32), ("graph", B2GraphInfo)]
 
 
 class B2TexError(RuntimeError):
@@ -223,6 +228,29 @@ class Context:
                    vv_ptr=np.zeros(self.Vn + 1, np.uint32), vv_idx=np.zeros(info.num_vertex_neighbours, np.uint32))
         _check(lib().b2tex_mesh_graph_download(self._h, *(_p(out[k]) for k in
                                                          ("adj_ptr", "adj_idx", "vf_ptr", "vf_idx", "vv_ptr", "vv_idx"))))
+        return out
+
+    def prepare_mesh(self, verts, faces) -> B2MeshPrepInfo:
+        """tex::prepare_mesh on the raw mesh (b2tex_prepare_mesh), e.g. the arrays of interchange.load_ply: drops the
+        redundant faces (face i goes when a face j > i has all its vertices among those of i), computes the face normals of
+        the kept faces, the mesh graph and the vertex normals.  Afterwards the context is as after set_mesh(verts, kept
+        faces, scene.face_normals of them) + build_mesh_graph; self.F is the kept count."""
+        v, f = _c(verts, np.float32), _c(faces, np.uint32)
+        info = B2MeshPrepInfo()
+        self.F = 0
+        _check(lib().b2tex_prepare_mesh(self._h, _p(v), C.c_uint32(v.shape[0]), _p(f), C.c_uint32(f.shape[0]),
+                                        C.byref(info)))
+        self.Vn, self.F = v.shape[0], int(info.num_faces)
+        return info
+
+    def prepared_mesh_download(self, info: B2MeshPrepInfo):
+        """dict(faces u32[F', 3], face_normals f32[F', 3], vertex_normals f32[Vn, 3], kept u32[F']): kept[i] is the input
+        id of face i, which maps per-face results back to the file's face ids"""
+        F = int(info.num_faces)
+        out = dict(faces=np.zeros((F, 3), np.uint32), face_normals=np.zeros((F, 3), np.float32),
+                   vertex_normals=np.zeros((self.Vn, 3), np.float32), kept=np.zeros(F, np.uint32))
+        _check(lib().b2tex_prepared_mesh_download(self._h, *(_p(out[k]) for k in
+                                                            ("faces", "face_normals", "vertex_normals", "kept"))))
         return out
 
     def set_num_faces(self, F):

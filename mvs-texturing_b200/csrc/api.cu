@@ -119,19 +119,61 @@ int b2tex_device_synchronize(b2tex_ctx *c)
     return B2TEX_OK;
 }
 
+}  // extern "C"
+
+// Uploads the vertices, the faces and (when given) the face normals and forgets everything derived from an earlier mesh.
+// The mesh is not marked valid: the caller does that.
+static int upload_mesh(b2tex_ctx *c, const float *verts, uint32_t nv, const uint32_t *faces, const float *normals,
+                       uint32_t nf)
+{
+    c->have_mesh = false; c->have_prep = false;
+    c->Vn = nv; c->F = nf; c->face_begin = 0; c->face_end = nf;
+    B2_TRY(c->verts.upload(verts, 3 * (size_t)nv, c->stream));
+    B2_TRY(c->faces.upload(faces, 3 * (size_t)nf, c->stream));
+    if (normals) B2_TRY(c->normals.upload(normals, 3 * (size_t)nf, c->stream));
+    B2_CUDA(cudaStreamSynchronize(c->stream));
+    c->bvh_built = false; c->have_costs = false; c->have_labels = false; c->have_adj = false;
+    c->have_rings = false; c->mrf_ready = false; c->have_seam = false;
+    return B2TEX_OK;
+}
+
+extern "C" {
+
 int b2tex_set_mesh(b2tex_ctx *c, const float *verts, uint32_t nv, const uint32_t *faces, const float *normals,
                    uint32_t nf)
 {
     B2_CUDA(cudaSetDevice(c->device));
     if (!verts || !faces || !normals) { set_error("set_mesh: null pointer"); return B2TEX_ERR_ARG; }
-    c->have_mesh = false;
-    c->Vn = nv; c->F = nf; c->face_begin = 0; c->face_end = nf;
-    B2_TRY(c->verts.upload(verts, 3 * (size_t)nv, c->stream));
-    B2_TRY(c->faces.upload(faces, 3 * (size_t)nf, c->stream));
-    B2_TRY(c->normals.upload(normals, 3 * (size_t)nf, c->stream));
+    B2_TRY(upload_mesh(c, verts, nv, faces, normals, nf));
+    c->have_mesh = true;
+    return B2TEX_OK;
+}
+
+int b2tex_prepare_mesh(b2tex_ctx *c, const float *verts, uint32_t nv, const uint32_t *faces, uint32_t nf,
+                       b2tex_mesh_prep_info *info)
+{
+    B2_CUDA(cudaSetDevice(c->device));
+    c->have_mesh = false; c->have_prep = false; c->have_adj = false; c->have_rings = false;
+    if (!verts || !faces) { set_error("prepare_mesh: null pointer"); return B2TEX_ERR_ARG; }
+    if (nf == 0) { set_error("prepare_mesh: the mesh has no faces"); return B2TEX_ERR_ARG; }
+    int rc = upload_mesh(c, verts, nv, faces, nullptr, nf);
+    if (rc == B2TEX_OK) rc = prepare_mesh(c, info);
+    if (rc != B2TEX_OK) {   // no mesh, graph or prepared arrays survive a failure
+        c->have_mesh = false; c->have_prep = false; c->have_adj = false; c->have_rings = false; c->mrf_ready = false;
+    }
+    return rc;
+}
+
+int b2tex_prepared_mesh_download(b2tex_ctx *c, uint32_t *faces, float *face_normals, float *vertex_normals,
+                                 uint32_t *kept_face_ids)
+{
+    B2_CUDA(cudaSetDevice(c->device));
+    if (!c->have_prep) { set_error("prepared_mesh_download: no prepared mesh is resident"); return B2TEX_ERR_ARG; }
+    if (faces) B2_TRY(c->faces.download(faces, 3 * (size_t)c->F, c->stream));
+    if (face_normals) B2_TRY(c->normals.download(face_normals, 3 * (size_t)c->F, c->stream));
+    if (vertex_normals) B2_TRY(c->vnormals.download(vertex_normals, 3 * (size_t)c->Vn, c->stream));
+    if (kept_face_ids) B2_TRY(c->kept_ids.download(kept_face_ids, c->F, c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
-    c->bvh_built = false; c->have_costs = false; c->have_labels = false; c->have_adj = false;
-    c->have_rings = false; c->mrf_ready = false; c->have_seam = false; c->have_mesh = true;
     return B2TEX_OK;
 }
 
@@ -509,7 +551,7 @@ static int acquire_ctx(b2tex_ctx **out)
                 b2tex_ctx *c = g_pool[i];
                 g_pool.erase(g_pool.begin() + (long)i);
                 c->have_costs = c->have_labels = c->have_adj = c->have_rings = c->mrf_ready = c->have_seam = false;
-                c->have_mesh = false;
+                c->have_mesh = false; c->have_prep = false;
                 c->images_prepared = false; c->prepared_data_term = -1; c->bvh_built = false;
                 c->Vn = c->F = c->K = 0; c->face_begin = c->face_end = 0; c->nnz = 0; c->R = 0;
                 *out = c;

@@ -157,6 +157,10 @@ struct b2tex_ctx {
     b2::DevBuf<float> verts, normals;
     b2::DevBuf<uint32_t> faces;
     bool have_mesh = false;   // set_mesh has run (view selection alone sets F without a mesh)
+    // prepare_mesh (prepare.cu): vertex normals [3 Vn] and the input id of every kept face [F]
+    b2::DevBuf<float> vnormals;
+    b2::DevBuf<uint32_t> kept_ids;
+    bool have_prep = false;   // the mesh came from a successful prepare_mesh
 
     // views
     uint32_t K = 0;
@@ -308,6 +312,10 @@ int patches_download(b2tex_ctx *c, int32_t *desc, uint32_t *faces, float *texcoo
 void patches_free(b2tex_ctx *c);
 int local_seam_run(b2tex_ctx *c, b2tex_local_seam_info *info);
 int build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info);
+// k_graph_validate: B2TEX_ERR_ARG naming the lowest face with an index >= nv ("<fn>: face ..."); sets up c->g_scal
+int validate_faces(b2tex_ctx *c, const uint32_t *faces, uint32_t F, uint32_t nv, const char *fn, const char *timer);
+// tex::prepare_mesh on the raw mesh resident in verts / faces (F, Vn set, have_mesh false)
+int prepare_mesh(b2tex_ctx *c, b2tex_mesh_prep_info *info);
 int cub_exclusive_sum_u64(b2tex_ctx *c, const uint64_t *in, uint64_t *out, size_t n);
 int cub_exclusive_sum_u32(b2tex_ctx *c, const uint32_t *in, uint32_t *out, size_t n);
 }  // namespace b2

@@ -226,24 +226,7 @@ int build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info)
     const unsigned grid = grid_of((size_t)F + 1);
     ScopedTimer total(c, "graph_build");   // the whole call, host round trips included
 
-    B2_TRY(c->g_scal.alloc(8));
-    unsigned long long init[8] = {GRAPH_NONE, 0, 0, 0, 0, 0, 0, 0};
-    B2_CUDA(cudaMemcpyAsync(c->g_scal.p, init, sizeof(init), cudaMemcpyHostToDevice, s));
-    {
-        ScopedTimer t(c, "graph_validate", 12.0 * F);
-        if (F) B2_LAUNCH k_graph_validate<<<grid, 256, 0, s>>>(c->faces.p, F, nv, c->g_scal.p);
-        B2_KERNEL_CHECK();
-    }
-    unsigned long long bad = GRAPH_NONE;
-    B2_CUDA(cudaMemcpyAsync(&bad, c->g_scal.p, sizeof(bad), cudaMemcpyDeviceToHost, s));
-    B2_CUDA(cudaStreamSynchronize(s));
-    if (bad != GRAPH_NONE) {
-        uint32_t fv[3];
-        B2_CUDA(cudaMemcpyAsync(fv, c->faces.p + 3 * (size_t)bad, sizeof(fv), cudaMemcpyDeviceToHost, s));
-        B2_CUDA(cudaStreamSynchronize(s));
-        set_error("build_mesh_graph: face %llu (%u %u %u) has a vertex index >= %u vertices", bad, fv[0], fv[1], fv[2], nv);
-        return B2TEX_ERR_ARG;
-    }
+    B2_TRY(validate_faces(c, c->faces.p, F, nv, "build_mesh_graph", "graph_validate"));
 
     B2_TRY(c->adj_ptr.alloc((size_t)F + 1));
     B2_TRY(c->vf_ptr.alloc((size_t)nv + 1));
@@ -348,6 +331,31 @@ int build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info)
         info->num_vertex_neighbours = (uint32_t)sc[4];
         info->max_face_degree = (uint32_t)sc[1];
         info->num_non_manifold_edges = (uint32_t)sc[2];
+    }
+    return B2TEX_OK;
+}
+
+int validate_faces(b2tex_ctx *c, const uint32_t *faces, uint32_t F, uint32_t nv, const char *fn, const char *timer)
+{
+    cudaStream_t s = c->stream;
+    const unsigned grid = (unsigned)std::min<size_t>(((size_t)F + 1 + 255) / 256 + 1, (size_t)c->num_sms * 16);
+    B2_TRY(c->g_scal.alloc(8));
+    unsigned long long init[8] = {GRAPH_NONE, 0, 0, 0, 0, 0, 0, 0};
+    B2_CUDA(cudaMemcpyAsync(c->g_scal.p, init, sizeof(init), cudaMemcpyHostToDevice, s));
+    {
+        ScopedTimer t(c, timer, 12.0 * F);
+        if (F) B2_LAUNCH k_graph_validate<<<grid, 256, 0, s>>>(faces, F, nv, c->g_scal.p);
+        B2_KERNEL_CHECK();
+    }
+    unsigned long long bad = GRAPH_NONE;
+    B2_CUDA(cudaMemcpyAsync(&bad, c->g_scal.p, sizeof(bad), cudaMemcpyDeviceToHost, s));
+    B2_CUDA(cudaStreamSynchronize(s));
+    if (bad != GRAPH_NONE) {
+        uint32_t fv[3];
+        B2_CUDA(cudaMemcpyAsync(fv, faces + 3 * (size_t)bad, sizeof(fv), cudaMemcpyDeviceToHost, s));
+        B2_CUDA(cudaStreamSynchronize(s));
+        set_error("%s: face %llu (%u %u %u) has a vertex index >= %u vertices", fn, bad, fv[0], fv[1], fv[2], nv);
+        return B2TEX_ERR_ARG;
     }
     return B2TEX_OK;
 }

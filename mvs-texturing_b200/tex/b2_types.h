@@ -53,12 +53,15 @@ public:
     FaceList &get_faces() { return faces; }
     NormalList const &get_face_normals() const { return face_normals; }
     NormalList &get_face_normals() { return face_normals; }
+    /* angle-weighted vertex normals, filled by tex::prepare_mesh (texrecon's OBJ writer reads them) */
+    NormalList const &get_vertex_normals() const { return vertex_normals; }
+    NormalList &get_vertex_normals() { return vertex_normals; }
     /* MVE ensure_normals(face=true): normalised cross(b-a, c-a), zero for degenerate faces */
     void ensure_face_normals();
 private:
     VertexList vertices;
     FaceList faces;
-    NormalList face_normals;
+    NormalList face_normals, vertex_normals;
 };
 
 /* mve::MeshInfo: per-vertex incident faces and 1-ring (global_seam_leveling.cpp:55,61,161,187) */

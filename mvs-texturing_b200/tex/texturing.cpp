@@ -11,6 +11,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <iostream>
 #include <limits>
 #include <mutex>
 
@@ -285,6 +286,38 @@ void DeviceSession::make_patches(mve::TriangleMesh::ConstPtr mesh, VertexProject
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+/* prepare_mesh.cpp:57-70 on a context of its own: no views exist yet when texrecon prepares the mesh (texrecon.cpp:79) */
+void prepare_mesh(mve::MeshInfo *mesh_info, mve::TriangleMesh::Ptr mesh)
+{
+    mve::TriangleMesh::FaceList &faces = mesh->get_faces();
+    std::size_t const F = faces.size() / 3, Vn = mesh->get_vertices().size();
+    if (F > std::numeric_limits<std::uint32_t>::max() || Vn > std::numeric_limits<std::uint32_t>::max())
+        throw std::runtime_error("Exeeded maximal number of faces");
+    {   /* a cached session of this mesh would describe the faces before the preparation */
+        std::lock_guard<std::mutex> lk(DeviceSession::mutex());
+        if (DeviceSession::cached() && DeviceSession::cached()->mesh_key == mesh.get()) DeviceSession::cached().reset();
+    }
+    int device = 0;
+    if (char const *e = std::getenv("B2TEX_DEVICE")) device = std::atoi(e);
+    b2tex_ctx *ctx = nullptr;
+    check(b2tex_create(device, &ctx));
+    std::shared_ptr<b2tex_ctx> owner(ctx, b2tex_destroy);
+    b2tex_mesh_prep_info info;
+    check(b2tex_prepare_mesh(ctx, Vn ? *mesh->get_vertices()[0] : nullptr, (std::uint32_t)Vn, faces.data(), (std::uint32_t)F,
+                             &info));
+    mve::TriangleMesh::NormalList &vn = mesh->get_vertex_normals();
+    bool const want_vertex = vn.size() != Vn;   /* ensure_normals recomputes only what is missing */
+    std::vector<std::uint32_t> kept_faces(3 * (std::size_t)info.num_faces);
+    mve::TriangleMesh::NormalList fn(info.num_faces);
+    if (want_vertex) vn.assign(Vn, math::Vec3f(0.0f));
+    check(b2tex_prepared_mesh_download(ctx, kept_faces.data(), info.num_faces ? *fn[0] : nullptr,
+                                       want_vertex && Vn ? *vn[0] : nullptr, nullptr));
+    if (info.num_redundant > 0) std::cout << "\tRemoved " << info.num_redundant << " redundant faces." << std::endl;
+    faces.assign(kept_faces.begin(), kept_faces.end());
+    mesh->get_face_normals().swap(fn);
+    mesh_info->initialize(mesh);
+}
+
 /* build_adjacency_graph.cpp:16-53 */
 void build_adjacency_graph(mve::TriangleMesh::ConstPtr mesh, mve::MeshInfo const &mesh_info, UniGraph *graph)
 {

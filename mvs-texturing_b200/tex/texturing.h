@@ -1,6 +1,7 @@
 // texturing.h -- the tex:: hot-path API of libs/tex/texturing.h:59-106 with the reference's signatures, backed by
 // libb2tex.so (include/b2tex.h):
 //
+//   prepare_mesh              texturing.h:46       b2tex_prepare_mesh            (redundant faces, face + vertex normals)
 //   build_adjacency_graph     texturing.h:59-61    host (feeds view_selection)
 //   calculate_data_costs      texturing.h:66-69    b2tex_data_costs_run          (costs stay on the GPU)
 //   postprocess_face_infos    texturing.h:71-74    b2tex_postprocess_face_infos
@@ -18,6 +19,11 @@
 #include "b2_types.h"
 
 namespace tex {
+
+/* texrecon.cpp:79: drops the redundant faces, sets the face normals of the kept faces and (when the mesh holds none) the
+ * vertex normals, re-initialises mesh_info and prints "\tRemoved N redundant faces." when N > 0 */
+void
+prepare_mesh(mve::MeshInfo * mesh_info, mve::TriangleMesh::Ptr mesh);
 
 void build_adjacency_graph(mve::TriangleMesh::ConstPtr mesh, mve::MeshInfo const &mesh_info, UniGraph *graph);
 
