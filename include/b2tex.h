@@ -146,7 +146,29 @@ int b2tex_profile(b2tex_ctx *ctx, int enable);
 int b2tex_profile_report(b2tex_ctx *ctx, char *buf, uint64_t cap);
 void b2tex_default_mrf_params(b2tex_mrf_params *p);
 
-/* ---- resident API: upload once, run stages on the device, download results ---- */
+/* ---- resident API: upload once, run stages on the device, download results ----
+ *
+ * A context holds uploads and the results derived from them.  An item stays valid until one it is derived from changes
+ * (transitively); a stage, or a download, whose inputs are not valid returns B2TEX_ERR_ARG and names them.
+ *
+ *   item             made valid by                                          derived from
+ *   mesh             set_mesh, prepare_mesh                                 -
+ *   prepared mesh    prepare_mesh (vertex normals, kept face ids)           mesh
+ *   BVH              the data-cost stage                                    mesh
+ *   face adjacency   set_adjacency, build_mesh_graph, prepare_mesh          mesh
+ *   vertex rings     set_vertex_rings, build_mesh_graph, prepare_mesh       mesh
+ *   views            set_views (cameras, number of views)                   -
+ *   pixels           set_views, undistort_views                             views
+ *   prepared images  the stages that read pixels                            pixels
+ *   data costs       data_costs_run / _normalize, set_data_costs            mesh, pixels; set_face_range invalidates them
+ *   view selection   mrf_init, view_selection_run (the state mrf_iterate,   data costs, face adjacency
+ *     state          mrf_energy and mrf_sample_forest read)
+ *   labels           set_labels, mrf_init, mrf_iterate, view_selection_run  mesh, views
+ *   seam system      seam_run, seam_assemble                                mesh, pixels, vertex rings, labels
+ *   seam solution    seam_run, seam_mg_solve                                seam system
+ *   texture patches  texture_patches_run                                    mesh, pixels, face adjacency, labels
+ *
+ * A stage invalidates its own result when it starts and marks it valid only when it succeeds. */
 int b2tex_set_mesh(b2tex_ctx *ctx, const float *verts, uint32_t num_verts, const uint32_t *faces,
                    const float *face_normals, uint32_t num_faces);
 int b2tex_set_views(b2tex_ctx *ctx, const b2tex_view *views, uint32_t num_views);
@@ -171,8 +193,8 @@ int b2tex_mesh_graph_download(b2tex_ctx *ctx, uint32_t *adj_ptr, uint32_t *adj_i
  * later degenerate face such as (a, a, b) uses only its vertices), the kept faces stay in their order, the vertices are
  * untouched.  Then the face normals of the kept faces (normalised cross(b - a, c - a), 0 when its length is 0), the mesh
  * graph (b2tex_build_mesh_graph) and angle-weighted vertex normals.  Afterwards the context is exactly as after
- * b2tex_set_mesh(verts, kept faces, their normals) + b2tex_build_mesh_graph, with the vertex normals resident; results of
- * earlier stages are discarded.  B2TEX_ERR_ARG for NULL pointers, num_faces == 0 or a face index >= num_verts (the first
+ * b2tex_set_mesh(verts, kept faces, their normals) + b2tex_build_mesh_graph, with the vertex normals resident.
+ * B2TEX_ERR_ARG for NULL pointers, num_faces == 0 or a face index >= num_verts (the first
  * such face is named); B2TEX_ERR_LIMITS when a count does not fit the 32-bit offsets.  A failure leaves no mesh.  info may
  * be NULL. */
 int b2tex_prepare_mesh(b2tex_ctx *ctx, const float *verts, uint32_t num_verts, const uint32_t *faces,
@@ -192,7 +214,7 @@ int b2tex_set_face_range(b2tex_ctx *ctx, uint32_t face_begin, uint32_t face_end)
  * undistorted pixels.  d[num_views], num_views == the number of views set.  Views with dist[0] == 0 stay untouched;
  * pixels whose source falls outside the image become 0 (and so may give the view a validity mask).  B2TEX_ERR_ARG if no
  * views are set, num_views differs, or a view to undistort has a focal length that is not finite and positive.  Call it
- * after b2tex_set_views and before the stages; results of earlier stages are discarded. */
+ * after b2tex_set_views and before the stages. */
 int b2tex_undistort_views(b2tex_ctx *ctx, const b2tex_distortion *d, uint32_t num_views);
 
 int b2tex_data_costs_run(b2tex_ctx *ctx, const b2tex_settings *settings, b2tex_dc_info *info);

@@ -126,14 +126,12 @@ int b2tex_device_synchronize(b2tex_ctx *c)
 static int upload_mesh(b2tex_ctx *c, const float *verts, uint32_t nv, const uint32_t *faces, const float *normals,
                        uint32_t nf)
 {
-    c->have_mesh = false; c->have_prep = false;
+    invalidate(c, MESH);
     c->Vn = nv; c->F = nf; c->face_begin = 0; c->face_end = nf;
     B2_TRY(c->verts.upload(verts, 3 * (size_t)nv, c->stream));
     B2_TRY(c->faces.upload(faces, 3 * (size_t)nf, c->stream));
     if (normals) B2_TRY(c->normals.upload(normals, 3 * (size_t)nf, c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
-    c->bvh_built = false; c->have_costs = false; c->have_labels = false; c->have_adj = false;
-    c->have_rings = false; c->mrf_ready = false; c->have_seam = false;
     return B2TEX_OK;
 }
 
@@ -145,7 +143,7 @@ int b2tex_set_mesh(b2tex_ctx *c, const float *verts, uint32_t nv, const uint32_t
     B2_CUDA(cudaSetDevice(c->device));
     if (!verts || !faces || !normals) { set_error("set_mesh: null pointer"); return B2TEX_ERR_ARG; }
     B2_TRY(upload_mesh(c, verts, nv, faces, normals, nf));
-    c->have_mesh = true;
+    mark_valid(c, MESH);
     return B2TEX_OK;
 }
 
@@ -153,14 +151,12 @@ int b2tex_prepare_mesh(b2tex_ctx *c, const float *verts, uint32_t nv, const uint
                        b2tex_mesh_prep_info *info)
 {
     B2_CUDA(cudaSetDevice(c->device));
-    c->have_mesh = false; c->have_prep = false; c->have_adj = false; c->have_rings = false;
+    invalidate(c, MESH);
     if (!verts || !faces) { set_error("prepare_mesh: null pointer"); return B2TEX_ERR_ARG; }
     if (nf == 0) { set_error("prepare_mesh: the mesh has no faces"); return B2TEX_ERR_ARG; }
     int rc = upload_mesh(c, verts, nv, faces, nullptr, nf);
     if (rc == B2TEX_OK) rc = prepare_mesh(c, info);
-    if (rc != B2TEX_OK) {   // no mesh, graph or prepared arrays survive a failure
-        c->have_mesh = false; c->have_prep = false; c->have_adj = false; c->have_rings = false; c->mrf_ready = false;
-    }
+    if (rc != B2TEX_OK) invalidate(c, MESH);   // no mesh, graph or prepared arrays survive a failure
     return rc;
 }
 
@@ -168,7 +164,7 @@ int b2tex_prepared_mesh_download(b2tex_ctx *c, uint32_t *faces, float *face_norm
                                  uint32_t *kept_face_ids)
 {
     B2_CUDA(cudaSetDevice(c->device));
-    if (!c->have_prep) { set_error("prepared_mesh_download: no prepared mesh is resident"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, PREP, "prepared_mesh_download"));
     if (faces) B2_TRY(c->faces.download(faces, 3 * (size_t)c->F, c->stream));
     if (face_normals) B2_TRY(c->normals.download(face_normals, 3 * (size_t)c->F, c->stream));
     if (vertex_normals) B2_TRY(c->vnormals.download(vertex_normals, 3 * (size_t)c->Vn, c->stream));
@@ -181,7 +177,7 @@ int b2tex_set_face_range(b2tex_ctx *c, uint32_t fb, uint32_t fe)
 {
     if (fb > fe || fe > c->F) { set_error("bad face range"); return B2TEX_ERR_ARG; }
     c->face_begin = fb; c->face_end = fe;
-    c->have_costs = false; c->mrf_ready = false;
+    invalidate(c, COSTS);
     return B2TEX_OK;
 }
 
@@ -189,6 +185,7 @@ int b2tex_set_views(b2tex_ctx *c, const b2tex_view *views, uint32_t K)
 {
     B2_CUDA(cudaSetDevice(c->device));
     if (K > 65535u) { set_error("Exeeded maximal number of views"); return B2TEX_ERR_LIMITS; }
+    invalidate(c, VIEWS);
     c->K = K;
     c->views_host.assign(views, views + K);
     c->img_off.assign((size_t)K + 1, 0);
@@ -223,7 +220,7 @@ int b2tex_set_views(b2tex_ctx *c, const b2tex_view *views, uint32_t K)
         B2_CUDA(cudaStreamSynchronize(c->stream));
         c->images_in_flight = false;
     }
-    c->images_prepared = false; c->prepared_data_term = -1; c->have_costs = false; c->have_seam = false;
+    mark_valid(c, VIEWS | PIXELS);
     return B2TEX_OK;
 }
 
@@ -237,10 +234,11 @@ int b2tex_set_adjacency(b2tex_ctx *c, const uint32_t *adj_ptr, const uint32_t *a
 {
     B2_CUDA(cudaSetDevice(c->device));
     if (!c->F) { set_error("set_adjacency: set the mesh (or data costs) first"); return B2TEX_ERR_ARG; }
+    invalidate(c, ADJ);
     B2_TRY(c->adj_ptr.upload(adj_ptr, (size_t)c->F + 1, c->stream));
     B2_TRY(c->adj_idx.upload(adj_idx, adj_ptr[c->F], c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
-    c->have_adj = true; c->mrf_ready = false;
+    mark_valid(c, ADJ);
     return B2TEX_OK;
 }
 
@@ -249,12 +247,13 @@ int b2tex_set_vertex_rings(b2tex_ctx *c, const uint32_t *vf_ptr, const uint32_t 
 {
     B2_CUDA(cudaSetDevice(c->device));
     if (!c->Vn) { set_error("set_vertex_rings: set the mesh first"); return B2TEX_ERR_ARG; }
+    invalidate(c, RINGS);
     B2_TRY(c->vf_ptr.upload(vf_ptr, (size_t)c->Vn + 1, c->stream));
     B2_TRY(c->vf_idx.upload(vf_idx, vf_ptr[c->Vn], c->stream));
     B2_TRY(c->vv_ptr.upload(vv_ptr, (size_t)c->Vn + 1, c->stream));
     B2_TRY(c->vv_idx.upload(vv_idx, vv_ptr[c->Vn], c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
-    c->have_rings = true;
+    mark_valid(c, RINGS);
     return B2TEX_OK;
 }
 
@@ -268,12 +267,9 @@ int b2tex_mesh_graph_download(b2tex_ctx *c, uint32_t *adj_ptr, uint32_t *adj_idx
                               uint32_t *vv_ptr, uint32_t *vv_idx)
 {
     B2_CUDA(cudaSetDevice(c->device));
-    if (!c->have_adj && !c->have_rings) { set_error("mesh_graph_download: no graph is resident"); return B2TEX_ERR_ARG; }
-    if ((adj_ptr || adj_idx) && !c->have_adj) { set_error("mesh_graph_download: no face adjacency is resident"); return B2TEX_ERR_ARG; }
-    if ((vf_ptr || vf_idx || vv_ptr || vv_idx) && !c->have_rings) {
-        set_error("mesh_graph_download: no vertex rings are resident");
-        return B2TEX_ERR_ARG;
-    }
+    if (!(c->valid & (ADJ | RINGS))) { set_error("mesh_graph_download: no graph is resident"); return B2TEX_ERR_ARG; }
+    if (adj_ptr || adj_idx) B2_TRY(require(c, ADJ, "mesh_graph_download"));
+    if (vf_ptr || vf_idx || vv_ptr || vv_idx) B2_TRY(require(c, RINGS, "mesh_graph_download"));
     if (adj_ptr) B2_TRY(c->adj_ptr.download(adj_ptr, (size_t)c->F + 1, c->stream));
     if (adj_idx) B2_TRY(c->adj_idx.download(adj_idx, c->adj_idx.n, c->stream));
     if (vf_ptr) B2_TRY(c->vf_ptr.download(vf_ptr, (size_t)c->Vn + 1, c->stream));
@@ -289,11 +285,13 @@ int b2tex_set_data_costs(b2tex_ctx *c, const uint64_t *face_ptr, const uint16_t 
     B2_CUDA(cudaSetDevice(c->device));
     if (!c->F) { set_error("set_data_costs: number of faces unknown (set mesh first)"); return B2TEX_ERR_ARG; }
     uint64_t nnz = face_ptr[c->F];
+    invalidate(c, COSTS);
     B2_TRY(c->dc_ptr.upload(face_ptr, (size_t)c->F + 1, c->stream));
     B2_TRY(c->dc_view.upload(view, nnz, c->stream));
     B2_TRY(c->dc_cost.upload(cost, nnz, c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
-    c->nnz = nnz; c->have_costs = true; c->mrf_ready = false;
+    c->nnz = nnz;
+    mark_valid(c, COSTS);
     return B2TEX_OK;
 }
 
@@ -303,9 +301,10 @@ int b2tex_set_labels(b2tex_ctx *c, const uint32_t *labels)
     if (c->K)   // texrecon.cpp:141-153 rejects such labelings ("Incorrect labeling"); the seam / patch kernels index views[label - 1]
         for (uint32_t i = 0; i < c->F; ++i)
             if (labels[i] > c->K) { set_error("Incorrect labeling (face %u has label %u, %u views)", i, labels[i], c->K); return B2TEX_ERR_LABELING; }
+    invalidate(c, LABELS);
     B2_TRY(c->labels.upload(labels, c->F, c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
-    c->have_labels = true;
+    mark_valid(c, LABELS);
     return B2TEX_OK;
 }
 
@@ -351,6 +350,7 @@ int b2tex_data_costs_run(b2tex_ctx *c, const b2tex_settings *st, b2tex_dc_info *
 int b2tex_data_costs_download(b2tex_ctx *c, uint64_t *face_ptr, uint16_t *view, float *cost, float *quality)
 {
     B2_CUDA(cudaSetDevice(c->device));
+    B2_TRY(require(c, COSTS, "data_costs_download"));
     if (face_ptr) B2_TRY(c->dc_ptr.download(face_ptr, (size_t)c->F + 1, c->stream));
     if (view) B2_TRY(c->dc_view.download(view, c->nnz, c->stream));
     if (cost) B2_TRY(c->dc_cost.download(cost, c->nnz, c->stream));
@@ -425,6 +425,7 @@ int b2tex_view_selection_run(b2tex_ctx *c, const b2tex_mrf_params *params, b2tex
 int b2tex_labels_download(b2tex_ctx *c, uint32_t *labels)
 {
     B2_CUDA(cudaSetDevice(c->device));
+    B2_TRY(require(c, LABELS, "labels_download"));
     B2_TRY(c->labels.download(labels, c->F, c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
     return B2TEX_OK;
@@ -485,7 +486,7 @@ int b2tex_seam_mg_solve(b2tex_ctx *c, b2tex_seam_info *info)
 int b2tex_seam_download(b2tex_ctx *c, uint32_t *row_ptr, uint32_t *row_label, float *x, float *rhs)
 {
     B2_CUDA(cudaSetDevice(c->device));
-    if (!c->have_seam) { set_error("seam_download before seam_run"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, SEAM, "seam_download"));
     const size_t R = c->R;
     if (row_ptr) B2_TRY(c->row_ptr.download(row_ptr, (size_t)c->Vn + 1, c->stream));
     if (row_label) B2_TRY(c->row_label.download(row_label, R, c->stream));
@@ -505,7 +506,7 @@ int b2tex_seam_download(b2tex_ctx *c, uint32_t *row_ptr, uint32_t *row_label, fl
 int b2tex_seam_matrix_download(b2tex_ctx *c, uint32_t *csr_ptr, uint32_t *csr_col, float *csr_val)
 {
     B2_CUDA(cudaSetDevice(c->device));
-    if (!c->have_seam) { set_error("seam_matrix_download before seam_run"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, SEAM, "seam_matrix_download"));
     B2_TRY(c->csr_ptr.download(csr_ptr, (size_t)c->R + 1, c->stream));
     B2_TRY(c->csr_col.download(csr_col, c->nnz_L, c->stream));
     B2_TRY(c->csr_val.download(csr_val, c->nnz_L, c->stream));
@@ -550,9 +551,7 @@ static int acquire_ctx(b2tex_ctx **out)
             if (g_pool[i]->device == device) {
                 b2tex_ctx *c = g_pool[i];
                 g_pool.erase(g_pool.begin() + (long)i);
-                c->have_costs = c->have_labels = c->have_adj = c->have_rings = c->mrf_ready = c->have_seam = false;
-                c->have_mesh = false; c->have_prep = false;
-                c->images_prepared = false; c->prepared_data_term = -1; c->bvh_built = false;
+                invalidate(c, ALL_ITEMS);
                 c->Vn = c->F = c->K = 0; c->face_begin = c->face_end = 0; c->nnz = 0; c->R = 0;
                 *out = c;
                 return B2TEX_OK;
@@ -668,7 +667,7 @@ int b2tex_view_selection(uint32_t nf, const uint32_t *adj_ptr, const uint32_t *a
 {
     b2tex_ctx *c = nullptr;
     B2_TRY(acquire_ctx(&c));
-    c->F = nf; c->face_begin = 0; c->face_end = nf;
+    set_face_count(c, nf);
     // DataCosts::rows() (= number of views) is not part of the CSR: params->num_views if the caller
     // knows it, otherwise bounded from the content (one host pass over nnz)
     uint32_t K = params ? params->num_views : 0;

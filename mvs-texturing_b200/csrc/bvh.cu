@@ -208,12 +208,13 @@ __global__ void k_refit(BvhNode *nodes, const int *__restrict__ parent_internal,
 
 int build_bvh(b2tex_ctx *c, bool force)
 {
-    if (c->bvh_built && !force) return B2TEX_OK;
+    if ((c->valid & BVH) && !force) return B2TEX_OK;
+    invalidate(c, BVH);
     ScopedTimer tm(c, "bvh_build");
     cudaStream_t s = c->stream;
     const uint32_t n = c->F;
     c->bvh.num_tris = n;
-    if (n == 0) { c->bvh_built = true; return B2TEX_OK; }
+    if (n == 0) { mark_valid(c, BVH); return B2TEX_OK; }
 
     DevBuf<uint32_t> &bnd = c->s_bnd, &ids_in = c->s_ids_in, &ids_out = c->s_ids_out, &counters = c->s_counters;
     DevBuf<uint64_t> &keys_in = c->s_keys_in, &keys_out = c->s_keys_out;
@@ -269,7 +270,7 @@ int build_bvh(b2tex_ctx *c, bool force)
         B2_KERNEL_CHECK();
     }
     B2_CUDA(cudaStreamSynchronize(s));
-    c->bvh_built = true;
+    mark_valid(c, BVH);
     return B2TEX_OK;
 }
 

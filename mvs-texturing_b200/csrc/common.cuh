@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "../../include/b2tex.h"
+#include "state.h"
 
 namespace b2 {
 
@@ -150,17 +151,16 @@ struct b2tex_ctx {
     cudaEvent_t images_uploaded = nullptr;
     bool defer_image_sync = false, images_in_flight = false;
     bool any_corner_flag = false;   // some view has a zero-sum corner pixel: validity masks exist and the cull reads them
+    uint32_t valid = 0;             // the items (state.h) that are up to date: invalidate / mark_valid / require below
 
     // mesh
     uint32_t Vn = 0, F = 0;
     uint32_t face_begin = 0, face_end = 0;
     b2::DevBuf<float> verts, normals;
     b2::DevBuf<uint32_t> faces;
-    bool have_mesh = false;   // set_mesh has run (view selection alone sets F without a mesh)
     // prepare_mesh (prepare.cu): vertex normals [3 Vn] and the input id of every kept face [F]
     b2::DevBuf<float> vnormals;
     b2::DevBuf<uint32_t> kept_ids;
-    bool have_prep = false;   // the mesh came from a successful prepare_mesh
 
     // views
     uint32_t K = 0;
@@ -168,12 +168,10 @@ struct b2tex_ctx {
     b2::DevBuf<uint8_t> rgb, grad, valid4;
     std::vector<size_t> img_off;          // pixel offset of each view in grad/valid4 (rgb: *3)
     b2::DevBuf<b2::ViewDev> views_dev;
-    bool images_prepared = false;
-    int prepared_data_term = -1;
+    int prepared_data_term = -1;          // the data term of the prepared images (while IMAGES is valid)
 
     // bvh
     b2::Bvh bvh;
-    bool bvh_built = false;
     b2::DevBuf<uint32_t> vrank, vorder;  // Morton rank of every vertex and its inverse
     // persistent scratch (grow only): cudaMalloc/cudaFree inside a stage would serialise the device
     b2::DevBuf<uint32_t> s_bnd, s_ids_in, s_ids_out, s_counters, s_vi_in, s_cnt32, s_row_vertex, s_rcnt, s_pass_bits, s_limits;
@@ -186,7 +184,6 @@ struct b2tex_ctx {
     b2::DevBuf<float> dc_cost;         // nnz
     b2::DevBuf<float> dc_quality;      // nnz
     uint64_t nnz = 0;
-    bool have_costs = false;
     // scratch of the data-cost stage
     b2::DevBuf<uint64_t> cand_ptr;     // F+1
     b2::DevBuf<uint16_t> cand_view;
@@ -202,7 +199,6 @@ struct b2tex_ctx {
     // graph + labels
     b2::DevBuf<uint32_t> adj_ptr, adj_idx;
     b2::DevBuf<uint32_t> labels;
-    bool have_adj = false, have_labels = false;
 
     // mrf scratch
     b2::DevBuf<float> mrf_H, mrf_hminp1;    // global-memory DP tables (trees that do not fit in shared memory only)
@@ -225,12 +221,10 @@ struct b2tex_ctx {
     unsigned long long mrf_forest_nodes = 0, mrf_forest_nnz = 0;   // summed over the iterations of the last run
     uint32_t mrf_slow_trees = 0;
     b2tex_mrf_params mrf_params{};
-    bool mrf_ready = false;
     int mrf_group = 32;
 
     // seam
     b2::DevBuf<uint32_t> vf_ptr, vf_idx, vv_ptr, vv_idx;
-    bool have_rings = false;
     // scratch of the mesh-graph build (graph.cu): sort keys [6F] x 2, values [3F] x 2, counts / run heads [6F], scalars
     b2::DevBuf<uint64_t> g_key[2];
     b2::DevBuf<uint32_t> g_val[2], g_cnt;
@@ -245,7 +239,6 @@ struct b2tex_ctx {
     b2::DevBuf<uint32_t> seam_status;
     uint32_t R = 0, A_rows = 0;
     uint64_t nnz_L = 0;
-    bool have_seam = false;
 
     // texture patches (allocated on first use, released by patches_free)
     b2::PatchState *patches = nullptr;
@@ -256,6 +249,28 @@ struct b2tex_ctx {
 };
 
 namespace b2 {
+// `bits` and everything derived from them are out of date
+inline void invalidate(b2tex_ctx *c, uint32_t bits) { c->valid &= ~(bits | dependents_of(bits)); }
+// `bits` were just (re)computed: everything derived from them is out of date, they are valid
+inline void mark_valid(b2tex_ctx *c, uint32_t bits) { c->valid = (c->valid & ~dependents_of(bits)) | bits; }
+// B2TEX_ERR_ARG naming the items of `bits` that are not valid
+inline int require(b2tex_ctx *c, uint32_t bits, const char *stage)
+{
+    const uint32_t missing = bits & ~c->valid;
+    if (!missing) return B2TEX_OK;
+    std::string names;
+    for (int i = 0; i < NUM_ITEMS; ++i)
+        if (missing & (1u << i)) names += std::string(names.empty() ? "" : ", ") + item_name(i);
+    set_error("%s: missing or out of date: %s", stage, names.c_str());
+    return B2TEX_ERR_ARG;
+}
+// F faces without a mesh (view selection or data-cost postprocessing of caller arrays)
+inline void set_face_count(b2tex_ctx *c, uint32_t F)
+{
+    invalidate(c, MESH);
+    c->F = F; c->face_begin = 0; c->face_end = F;
+}
+
 // Records a pair of events around a launch sequence on the context's stream when profiling is on.
 struct ScopedTimer {
     b2tex_ctx *c;
@@ -314,7 +329,7 @@ int local_seam_run(b2tex_ctx *c, b2tex_local_seam_info *info);
 int build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info);
 // k_graph_validate: B2TEX_ERR_ARG naming the lowest face with an index >= nv ("<fn>: face ..."); sets up c->g_scal
 int validate_faces(b2tex_ctx *c, const uint32_t *faces, uint32_t F, uint32_t nv, const char *fn, const char *timer);
-// tex::prepare_mesh on the raw mesh resident in verts / faces (F, Vn set, have_mesh false)
+// tex::prepare_mesh on the raw mesh resident in verts / faces (F, Vn set, MESH not valid)
 int prepare_mesh(b2tex_ctx *c, b2tex_mesh_prep_info *info);
 int cub_exclusive_sum_u64(b2tex_ctx *c, const uint64_t *in, uint64_t *out, size_t n);
 int cub_exclusive_sum_u32(b2tex_ctx *c, const uint32_t *in, uint32_t *out, size_t n);

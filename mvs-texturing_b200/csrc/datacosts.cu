@@ -689,13 +689,14 @@ static int finish_candidates(b2tex_ctx *c, const b2tex_settings *st, uint64_t nu
     info->rays = rays;
     info->max_quality = maxq;
     info->percentile = 0.0f;
-    c->have_costs = false;
     return B2TEX_OK;
 }
 
 int data_costs_qualities(b2tex_ctx *c, const b2tex_settings *st, b2tex_dc_info *info)
 {
+    invalidate(c, COSTS);
     if (!c->F || !c->K) { set_error("data costs: mesh and views must be set first"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, MESH | PIXELS, "data costs"));
     if (st->outlier_removal < 0 || st->outlier_removal > 2) { set_error("unknown outlier removal mode"); return B2TEX_ERR_UNSUPPORTED; }
     const bool outlier = st->outlier_removal != 0;
     if (c->K > 65535u) { set_error("Exeeded maximal number of views"); return B2TEX_ERR_LIMITS; }
@@ -802,7 +803,7 @@ int data_costs_postprocess(b2tex_ctx *c, const b2tex_settings *st, uint32_t F, c
     const bool outlier = st->outlier_removal != 0;
     if (outlier && !mean_ycbcr) { set_error("postprocess_face_infos: outlier removal needs the mean colours"); return B2TEX_ERR_ARG; }
     cudaStream_t s = c->stream;
-    c->F = F; c->face_begin = 0; c->face_end = F;
+    set_face_count(c, F);
     const uint64_t n = face_ptr[F];
     B2_TRY(c->cand_ptr.upload(face_ptr, (size_t)F + 1, s));
     B2_TRY(c->cand_view.upload(view, n, s));
@@ -853,8 +854,7 @@ int data_costs_normalize(b2tex_ctx *c, float gmax, const uint32_t *bins, b2tex_d
     info->nnz = c->nnz;
     info->max_quality = gmax;
     info->percentile = percentile;
-    c->have_costs = true;
-    c->mrf_ready = false;
+    mark_valid(c, COSTS);
     return B2TEX_OK;
 }
 

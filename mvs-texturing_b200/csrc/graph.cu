@@ -212,9 +212,8 @@ __global__ void k_graph_vv_scatter(const uint64_t *key, const uint32_t *head, co
 int build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info)
 {
     cudaStream_t s = c->stream;
-    // a failed build leaves no graph behind
-    c->have_adj = false; c->have_rings = false; c->mrf_ready = false;
-    if (!c->have_mesh) { set_error("build_mesh_graph: set the mesh first"); return B2TEX_ERR_ARG; }
+    invalidate(c, ADJ | RINGS);   // a failed build leaves no graph behind
+    B2_TRY(require(c, MESH, "build_mesh_graph"));
     const uint32_t F = c->F, nv = c->Vn;
     if (6ull * F > 0x7FFFFFFFull) {
         set_error("build_mesh_graph: %u faces exceed the sort's 32-bit item count (at most %u)", F, 0x7FFFFFFFu / 6);
@@ -235,7 +234,7 @@ int build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info)
         B2_TRY(c->adj_idx.alloc(0)); B2_TRY(c->vf_idx.alloc(0)); B2_TRY(c->vv_idx.alloc(0));
         B2_TRY(c->adj_ptr.zero(s)); B2_TRY(c->vf_ptr.zero(s)); B2_TRY(c->vv_ptr.zero(s));
         B2_CUDA(cudaStreamSynchronize(s));
-        c->have_adj = c->have_rings = true;
+        mark_valid(c, ADJ | RINGS);
         if (info) *info = b2tex_graph_info{0, 0, 0, 0, 0};
         return B2TEX_OK;
     }
@@ -324,7 +323,7 @@ int build_mesh_graph(b2tex_ctx *c, b2tex_graph_info *info)
     B2_CUDA(cudaMemcpyAsync(sc, c->g_scal.p, sizeof(sc), cudaMemcpyDeviceToHost, s));
     B2_CUDA(cudaStreamSynchronize(s));
     c->vv_idx.n = (size_t)sc[4];
-    c->have_adj = true; c->have_rings = true;
+    mark_valid(c, ADJ | RINGS);
     if (info) {
         info->num_adjacency = num_adj;
         info->num_vertex_faces = n3;

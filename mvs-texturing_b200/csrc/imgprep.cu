@@ -437,8 +437,9 @@ int prepare_views(b2tex_ctx *c, int data_term)
 
 int prepare_images(b2tex_ctx *c, int data_term, bool force)
 {
-    if (!force && c->images_prepared && c->prepared_data_term == data_term) return B2TEX_OK;
+    if (!force && (c->valid & IMAGES) && c->prepared_data_term == data_term) return B2TEX_OK;
     if (!c->K) { set_error("prepare_images: no views set"); return B2TEX_ERR_ARG; }
+    invalidate(c, IMAGES);
     B2_TRY(wait_for_images(c));
     cudaStream_t s = c->stream;
     const uint32_t K = c->K;
@@ -525,8 +526,8 @@ int prepare_images(b2tex_ctx *c, int data_term, bool force)
     } else {
         B2_CUDA(cudaStreamSynchronize(s));
     }
-    c->images_prepared = true;
     c->prepared_data_term = data_term;
+    mark_valid(c, IMAGES);
     return B2TEX_OK;
 }
 

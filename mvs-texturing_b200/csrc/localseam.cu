@@ -620,7 +620,7 @@ __global__ void __launch_bounds__(256) k_poisson_write(uint64_t P, const uint8_t
 
 int local_seam_run(b2tex_ctx *c, b2tex_local_seam_info *info)
 {
-    if (!c->patches || !c->patches->ready) { set_error("local seam leveling: run b2tex_texture_patches_run first"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, PATCHES, "local seam leveling"));
     PatchState &ps = *c->patches;
     if (ps.leveled) { set_error("local seam leveling was already applied to these patches"); return B2TEX_ERR_ARG; }
     cudaStream_t s = c->stream;
@@ -636,7 +636,7 @@ int local_seam_run(b2tex_ctx *c, b2tex_local_seam_info *info)
     uint32_t NE = 0, S = 0, NV = 0, NL = 0, NVP = 0;
     static const bool plan_on_host = getenv("B2TEX_LSEAM_HOST") != nullptr;   // diagnostic: the host bookkeeping of patches_host.h
     bool planned = false;
-    if (c->have_rings && !plan_on_host && T && F < 0x7FFFFFFFu) {
+    if ((c->valid & RINGS) && !plan_on_host && T && F < 0x7FFFFFFFu) {
         ScopedTimer t_plan(c, "ls.plan_on_device");
         const uint32_t Vn = c->Vn;
         DevBuf<uint32_t> &face_slot = ps.plan_face_slot, &cnt_a = ps.plan_cnt_a, &cnt_b = ps.plan_cnt_b, &off_a = ps.plan_off_a,

@@ -1190,8 +1190,7 @@ int enqueue_iteration(b2tex_ctx *c, Mrf &m, bool stop_rule)
 
 int alloc_mrf(b2tex_ctx *c, const b2tex_mrf_params *p)
 {
-    if (!c->have_costs) { set_error("view selection: data costs missing"); return B2TEX_ERR_ARG; }
-    if (!c->have_adj) { set_error("view selection: adjacency missing"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, COSTS | ADJ, "view selection"));
     if (p->rounds + 2 > (uint32_t)MAX_LEVELS) { set_error("mrf rounds too large"); return B2TEX_ERR_ARG; }
     if (p->max_iterations + 4 > MRF_SLOTS) { set_error("view selection: at most %u iterations", MRF_SLOTS - 4); return B2TEX_ERR_ARG; }
     c->mrf_params = *p;
@@ -1239,7 +1238,7 @@ int alloc_mrf(b2tex_ctx *c, const b2tex_mrf_params *p)
     if (forest_timing) { B2_TRY(c->mrf_dbg.alloc(16)); B2_TRY(c->mrf_dbg.zero(c->stream)); }
     B2_TRY(c->mrf_adj4.alloc(F));
     if (F) B2_LAUNCH k_build_adj4<<<(unsigned)((F + 255) / 256), 256, 0, c->stream>>>((uint32_t)F, c->adj_ptr.p, c->adj_idx.p, c->mrf_adj4.p);
-    if (!c->have_labels || c->labels.n != F) { B2_TRY(c->labels.alloc(F)); B2_TRY(c->labels.zero(c->stream)); }
+    if (!(c->valid & LABELS) || c->labels.n != F) { B2_TRY(c->labels.alloc(F)); B2_TRY(c->labels.zero(c->stream)); }
     uint32_t nodes = c->face_end - c->face_begin;
     double rho = nodes ? (double)c->nnz / nodes : 0.0;
     // lanes per node: a level of one tree holds only a few nodes, so wide groups idle on short label lists
@@ -1289,7 +1288,9 @@ int read_energy(b2tex_ctx *c, const Mrf &m, uint32_t slot, int64_t *efix)
 // init: arg-min labels of the owned faces, (multi-GPU: boundary labels to the peers,) energy of the initial labeling
 int mrf_init(b2tex_ctx *c, const b2tex_mrf_params *p, int64_t *efix)
 {
-    B2_TRY(alloc_mrf(c, p));
+    invalidate(c, MRF);
+    B2_TRY(alloc_mrf(c, p));   // keeps the labels of faces outside the owned range while they are valid
+    invalidate(c, LABELS);
     Mrf m = make_mrf(c, 0);
     cudaStream_t s = c->stream;
     const int grid = std::max(1, c->num_sms * 8);
@@ -1314,10 +1315,10 @@ int mrf_init(b2tex_ctx *c, const b2tex_mrf_params *p, int64_t *efix)
         }
         B2_KERNEL_CHECK();
     }
-    c->have_labels = true;
-    c->mrf_ready = true;
     if (m.ne > m.nb || mg_active(c)) B2_TRY(enqueue_exchange_and_energy(c, m, 0u, false));
-    return read_energy(c, m, 0u, efix);
+    B2_TRY(read_energy(c, m, 0u, efix));
+    mark_valid(c, LABELS | MRF);
+    return B2TEX_OK;
 }
 
 // every allocation of a run, nothing else: a caller that drives several ranks from ONE process (threads) prepares all of
@@ -1342,13 +1343,16 @@ int mrf_prepare(b2tex_ctx *c, const b2tex_mrf_params *p)
 // one iteration, energy read back (single GPU, or the building block of a host-driven sharded loop over NCCL)
 int mrf_iterate(b2tex_ctx *c, uint32_t t, int64_t *efix)
 {
-    if (!c->mrf_ready) { set_error("mrf_iterate before mrf_init"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, MRF, "mrf_iterate"));
     if (t == 0 || t > c->mrf_params.max_iterations) { set_error("mrf_iterate: iterations are numbered from 1 to max_iterations"); return B2TEX_ERR_ARG; }
+    invalidate(c, LABELS);
     Mrf m = make_mrf(c, t);
     B2_CUDA(cudaMemsetAsync(m.efix + t, 0, sizeof(unsigned long long), c->stream));
     if (mg_active(c)) B2_CUDA(cudaMemsetAsync(c->mrf_mg->elocal.p + t, 0, sizeof(unsigned long long), c->stream));
     B2_TRY(enqueue_iteration(c, m, false));
-    return read_energy(c, m, t, efix);
+    B2_TRY(read_energy(c, m, t, efix));
+    mark_valid(c, LABELS);
+    return B2TEX_OK;
 }
 
 // The whole run without a host round trip per iteration: the host queues iterations ahead of the device; the stop rule
@@ -1369,6 +1373,7 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
         if (trace) for (uint32_t t = 0; t <= t_end; ++t) trace[t] = info->energy_initial;
         return B2TEX_OK;
     }
+    invalidate(c, LABELS);   // until the iterations below have finished without error
     constexpr int LAG = 3;   // iterations queued beyond the last one whose stop flag the host has seen
     cudaEvent_t ev[LAG + 1];
     for (auto &e : ev) B2_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -1443,6 +1448,7 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
         fprintf(stderr, "k_tree: trees through global memory %u, forest nodes %llu in %llu labels\n", st[ST_SLOW], fn, fz);
     }
     if (st[ST_BAD]) { set_error("Incorrect labeling"); return B2TEX_ERR_LABELING; }
+    mark_valid(c, LABELS);
     return B2TEX_OK;
 }
 
@@ -1450,7 +1456,7 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
 // this after its own label exchange, so that cut edges see the neighbours' NEW labels)
 int mrf_energy_only(b2tex_ctx *c, int64_t *efix)
 {
-    if (!c->mrf_ready) { set_error("mrf_energy before mrf_init"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, MRF, "mrf_energy"));
     Mrf m = make_mrf(c, 1);
     const uint32_t slot = MRF_SLOTS - 1;   // scratch slot
     B2_CUDA(cudaMemsetAsync(m.efix + slot, 0, sizeof(unsigned long long), c->stream));
@@ -1461,7 +1467,7 @@ int mrf_energy_only(b2tex_ctx *c, int64_t *efix)
 
 int mrf_sample_only(b2tex_ctx *c, const b2tex_mrf_params *p, uint32_t t, uint32_t *level_host)
 {
-    if (!c->mrf_ready) { int64_t e; B2_TRY(mrf_init(c, p, &e)); }
+    if (!(c->valid & MRF)) { int64_t e; B2_TRY(mrf_init(c, p, &e)); }
     c->mrf_params = *p;
     Mrf m = make_mrf(c, t);
     B2_TRY(c->mrf_queue.zero(c->stream));  // the same (iteration, round) stamps may be replayed
@@ -1476,7 +1482,7 @@ void mrf_mg_free(b2tex_ctx *c)
 {
     MrfMgState *g = c->mrf_mg;
     if (!g) return;
-    if (c->labels.borrowed) { c->labels.release(); c->have_labels = false; }
+    if (c->labels.borrowed) { c->labels.release(); invalidate(c, LABELS); }
     for (uint32_t k = 0; k < (uint32_t)MRF_MAX_RANKS; ++k)
         if (g->opened[k] && g->peer[k]) cudaIpcCloseMemHandle(g->peer[k]);
     if (g->block) cudaFree(g->block);
@@ -1499,7 +1505,7 @@ int mrf_mg_export(b2tex_ctx *c, uint32_t rank, uint32_t nranks, void *handle64)
     B2_CUDA(cudaStreamSynchronize(c->stream));
     g->peer[rank] = g->block;
     c->labels.borrow((uint32_t *)g->block, c->F);
-    c->have_labels = false;
+    invalidate(c, LABELS);
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
     cudaIpcMemHandle_t h;
     memset(&h, 0, sizeof(h));

@@ -259,16 +259,14 @@ void patches_free(b2tex_ctx *c)
 
 int patches_run(b2tex_ctx *c, int apply_adjust, b2tex_patch_info *info)
 {
-    if (!c->F || !c->K || !c->have_adj || !c->have_labels) {
-        set_error("texture patches: mesh, views, adjacency and labels must be set");
-        return B2TEX_ERR_ARG;
-    }
-    if (apply_adjust && !c->have_seam) { set_error("texture patches: run the seam leveling first (or pass apply_adjust = 0)"); return B2TEX_ERR_ARG; }
+    invalidate(c, PATCHES);
+    if (!c->F || !c->K) { set_error("texture patches: mesh, views, adjacency and labels must be set"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, MESH | PIXELS | ADJ | LABELS, "texture patches"));
+    if (apply_adjust) B2_TRY(require(c, SEAM, "texture patches with apply_adjust (or pass apply_adjust = 0)"));
     cudaStream_t s = c->stream;
-    B2_TRY(prepare_images(c, c->prepared_data_term >= 0 ? c->prepared_data_term : 0));
+    B2_TRY(prepare_images(c, (c->valid & IMAGES) ? c->prepared_data_term : 0));
     if (!c->patches) c->patches = new PatchState();
     PatchState &ps = *c->patches;
-    ps.ready = false;
     ps.leveled = false;
     ScopedTimer tm(c, "texture_patches");
 
@@ -356,14 +354,14 @@ int patches_run(b2tex_ctx *c, int apply_adjust, b2tex_patch_info *info)
     info->num_patches = NP;
     info->num_faces = T;
     info->num_pixels = P;
-    ps.ready = true;
+    mark_valid(c, PATCHES);
     return B2TEX_OK;
 }
 
 int patches_download(b2tex_ctx *c, int32_t *desc, uint32_t *faces, float *texcoords, float *images, uint8_t *validity,
                      uint8_t *blending)
 {
-    if (!c->patches || !c->patches->ready) { set_error("texture_patches_download before texture_patches_run"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, PATCHES, "texture_patches_download"));
     PatchState &ps = *c->patches;
     cudaStream_t s = c->stream;
     const size_t T = ps.faces.size();

@@ -14,7 +14,6 @@ struct PatchState {
     DevBuf<float> px, tex, chain, adj, img;
     DevBuf<uint8_t> valid, blend;
     uint64_t total_pixels = 0;
-    bool ready = false;
     // local seam leveling (localseam.cu)
     DevBuf<float> orig;                   // images before the seam colours are stamped (Poisson source)
     DevBuf<float> edge_proj, edge_color, vert_color, vert_proj;

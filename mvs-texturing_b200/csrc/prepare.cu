@@ -268,7 +268,7 @@ int prepare_mesh(b2tex_ctx *c, b2tex_mesh_prep_info *info)
     B2_CUDA(cudaStreamSynchronize(s));
     c->faces.n = 3 * (size_t)Fk; c->normals.n = 3 * (size_t)Fk; c->kept_ids.n = Fk;
     c->F = Fk; c->face_begin = 0; c->face_end = Fk;
-    c->have_mesh = true;
+    mark_valid(c, MESH);
 
     b2tex_graph_info gi;
     B2_TRY(build_mesh_graph(c, &gi));
@@ -280,7 +280,7 @@ int prepare_mesh(b2tex_ctx *c, b2tex_mesh_prep_info *info)
         B2_KERNEL_CHECK();
     }
     B2_CUDA(cudaStreamSynchronize(s));
-    c->have_prep = true;
+    mark_valid(c, PREP);
     if (info) {
         info->num_faces_in = F;
         info->num_faces = Fk;

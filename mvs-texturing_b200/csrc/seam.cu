@@ -532,13 +532,12 @@ __global__ void __launch_bounds__(PCG_THREADS, 1) k_pcg(Pcg q)
 
 int seam_run(b2tex_ctx *c, b2tex_seam_info *info, bool solve)
 {
-    if (!c->Vn || !c->have_rings || !c->have_labels || !c->K) {
-        set_error("seam leveling: mesh, vertex rings, labels and views must be set");
-        return B2TEX_ERR_ARG;
-    }
+    invalidate(c, SEAM_SYSTEM);
+    if (!c->Vn || !c->K) { set_error("seam leveling: mesh, vertex rings, labels and views must be set"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, MESH | PIXELS | RINGS | LABELS, "seam leveling"));
     cudaStream_t s = c->stream;
     // only the camera block and the rgb images are needed here (no gradient image)
-    B2_TRY(prepare_images(c, c->prepared_data_term >= 0 ? c->prepared_data_term : 0));
+    B2_TRY(prepare_images(c, (c->valid & IMAGES) ? c->prepared_data_term : 0));
     const uint32_t Vn = c->Vn;
     std::unique_ptr<ScopedTimer> tm_asm(new ScopedTimer(c, "seam_assembly"));
     DevBuf<uint32_t> &cnt = c->s_cnt32, &row_vertex = c->s_row_vertex;
@@ -614,6 +613,7 @@ int seam_run(b2tex_ctx *c, b2tex_seam_info *info, bool solve)
                                           c->csr_ptr.p, c->csr_col.p, c->csr_val.p, c->seam_diag.p, c->seam_rhs.p, c->csr_enc.p,
                                           c->seam_dval.p);
     B2_KERNEL_CHECK();
+    mark_valid(c, SEAM_SYSTEM);
 
     // Gamma rows = sum over rows of Gamma neighbours / 2
     info->num_rows = R;
@@ -666,7 +666,7 @@ int seam_run(b2tex_ctx *c, b2tex_seam_info *info, bool solve)
         info->cg_launch_iterations = st[6];
         info->cg_ms = ms;
     }
-    c->have_seam = solve;
+    if (solve) mark_valid(c, SEAM);
     return B2TEX_OK;
 }
 

@@ -546,6 +546,8 @@ void *seam_mg_block(b2tex_ctx *c) { return c->seam_mg ? c->seam_mg->block : null
 
 int seam_mg_solve(b2tex_ctx *c, b2tex_seam_info *info)
 {
+    invalidate(c, SEAM);
+    B2_TRY(require(c, SEAM_SYSTEM, "seam_mg_solve"));
     MgState *m = c->seam_mg;
     if (!m || m->R != c->R) { set_error("seam_mg_solve: export / import the peer blocks for this system first"); return B2TEX_ERR_ARG; }
     for (uint32_t k = 0; k < m->nranks; ++k)
@@ -601,7 +603,7 @@ int seam_mg_solve(b2tex_ctx *c, b2tex_seam_info *info)
     for (int ch = 0; ch < 3; ++ch) { info->iterations[ch] = st[ch]; memcpy(&info->residual[ch], &st[3 + ch], 4); }
     info->cg_launch_iterations = st[6];
     info->cg_ms = ms;
-    c->have_seam = true;
+    mark_valid(c, SEAM);
     return B2TEX_OK;
 }
 

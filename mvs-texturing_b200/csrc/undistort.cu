@@ -93,6 +93,7 @@ constexpr size_t UNDISTORT_SCRATCH_BYTES = size_t(256) << 20;
 int undistort_views(b2tex_ctx *c, const b2tex_distortion *d, uint32_t num_views)
 {
     if (!c->K) { set_error("undistort_views: no views set"); return B2TEX_ERR_ARG; }
+    B2_TRY(require(c, PIXELS, "undistort_views"));
     if (num_views != c->K) { set_error("undistort_views: %u distortions for %u views", num_views, c->K); return B2TEX_ERR_ARG; }
     if (!d) { set_error("undistort_views: null distortion array"); return B2TEX_ERR_ARG; }
     std::vector<uint32_t> todo;
@@ -106,6 +107,7 @@ int undistort_views(b2tex_ctx *c, const b2tex_distortion *d, uint32_t num_views)
         todo.push_back(v);
     }
     if (todo.empty()) return B2TEX_OK;
+    invalidate(c, PIXELS);
     B2_TRY(wait_for_images(c));
     cudaStream_t s = c->stream;
 
@@ -160,7 +162,7 @@ int undistort_views(b2tex_ctx *c, const b2tex_distortion *d, uint32_t num_views)
     B2_TRY(prepare_views(c, 0));
     B2_TRY(zero_corner_flags(c, flags));   // synchronises the stream: scratch and dv may go
     c->any_corner_flag = std::any_of(flags.begin(), flags.end(), [](uint32_t f) { return f != 0; });
-    c->images_prepared = false; c->prepared_data_term = -1; c->have_costs = false; c->have_seam = false;
+    mark_valid(c, PIXELS);
     return B2TEX_OK;
 }
 

@@ -109,7 +109,6 @@ public:
     std::shared_ptr<std::vector<float> > images;
     std::shared_ptr<std::vector<std::uint8_t> > validity, blending;
     bool pixels_stale = false;   // the device holds newer patch pixels than the mirrors
-    bool have_seam = false;
     b2tex_seam_info seam_info{};
 
     ~DeviceSession() { if (ctx) b2tex_destroy(ctx); }
@@ -417,7 +416,6 @@ void generate_texture_patches(UniGraph const &graph, mve::TriangleMesh::ConstPtr
     s->set_graph(graph);
     s->set_rings(mesh_info);
     s->set_labels(graph);   // always: the labeling may come from a file (-L, texrecon.cpp:137-158)
-    s->have_seam = false;
     /* crop + the zero-offset adjust_colors pass of texrecon.cpp:174-183 (validity / blending masks); global_seam_leveling
      * re-crops and applies the solved offsets */
     check(b2tex_texture_patches_run(s->ctx, 0, &s->pinfo));
@@ -439,7 +437,6 @@ void global_seam_leveling(UniGraph const &, mve::TriangleMesh::ConstPtr, mve::Me
     /* labels, rings and patches are resident since generate_texture_patches: assemble + solve (global_seam_leveling.cpp:
      * 150-291), then adjust_colors of every patch with the solved offsets (:293-323) */
     check(b2tex_seam_run(s->ctx, &s->seam_info));
-    s->have_seam = true;
     b2tex_patch_info pi;
     check(b2tex_texture_patches_run(s->ctx, 1, &pi));
     if (pi.num_patches != s->pinfo.num_patches || pi.num_pixels != s->pinfo.num_pixels)
@@ -459,7 +456,6 @@ void local_seam_leveling(UniGraph const &, mve::TriangleMesh::ConstPtr, VertexPr
 void get_adjust_values(TexturePatches const &texture_patches, AdjustValues *adjust_values)
 {
     std::shared_ptr<DeviceSession> s = session_of(texture_patches);
-    if (!s->have_seam) throw std::runtime_error("tex::get_adjust_values: run tex::global_seam_leveling first");
     std::size_t const R = s->seam_info.num_rows;
     std::vector<std::uint32_t> row_ptr(s->Vn + 1), row_label(std::max<std::size_t>(R, 1));
     std::vector<float> x(3 * std::max<std::size_t>(R, 1));
