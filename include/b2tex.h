@@ -71,6 +71,10 @@ typedef struct {
     float ratio;
     uint32_t num_parts;    /* logical face partitions (>=1); >1 reproduces the multi-GPU schedule */
     uint32_t num_views;    /* DataCosts::rows() for the one-shot call; 0 = derive from the entries */
+    uint32_t use_multilevel;   /* mapMAP_control::use_multilevel: after the stop rule fires, contract every same-label
+                                  region into one node, solve the contracted MRF (weighted Potts) from the current labels
+                                  and go back to the faces while that lowers the energy.  One GPU, whole mesh, num_parts 1
+                                  only (else B2TEX_ERR_UNSUPPORTED).  Default 0. */
 } b2tex_mrf_params;
 
 typedef struct {
@@ -79,6 +83,8 @@ typedef struct {
     double energy_final;
     uint64_t unseen;       /* "faces have not been seen" view_selection.cpp:132 */
     uint64_t sweep_bytes;  /* algorithmic bytes of one sweep (SURVEY 8d): 14 nnz + 20 F */
+    uint32_t multilevel_passes;   /* use_multilevel: contractions whose coarse solve lowered the energy */
+    uint32_t coarse_nodes;        /* use_multilevel: nodes of the last contraction */
 } b2tex_mrf_info;
 
 typedef struct {

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb2tex.so")
 SOURCES = ["api.cu", "imgprep.cu", "bvh.cu", "datacosts.cu", "mrf.cu", "seam.cu", "patches.cu", "localseam.cu", "seam_mg.cu",
-           "undistort.cu", "graph.cu", "prepare.cu"]
+           "undistort.cu", "graph.cu", "prepare.cu", "mrf_multilevel.cu"]
 # -fmad=false: results must match the fp32 operation order of the reference restatement (oracle/)
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-fmad=false", "-Xcompiler", "-fPIC", "-Xcompiler", "-O3", "-Xptxas", "-v",

@@ -38,6 +38,7 @@ void b2tex_default_mrf_params(b2tex_mrf_params *p)
     p->ratio = 0.01f;
     p->num_parts = 1;
     p->num_views = 0;
+    p->use_multilevel = 0;
 }
 
 int b2tex_create(int device, b2tex_ctx **out)

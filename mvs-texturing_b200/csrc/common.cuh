@@ -217,6 +217,18 @@ struct b2tex_ctx {
     b2::DevBuf<uint4> mrf_rec;         // [3 F] 48-byte node records in forest order (k_tree_prep)
     b2::DevBuf<uint4> mrf_adj4;        // compact degree<=3 adjacency
     b2::DevBuf<uint32_t> mrf_queue;    // forest frontier lists + stamps
+    // the contracted MRF of multilevel view selection (mrf_multilevel.cu), grow-only scratch: node of every face, per node
+    // label / label position / size / label-list offsets / CSR row / compact adjacency, coarse label lists and edges, and the
+    // sort and scan buffers of the contraction (max(nnz, adjacency entries) each)
+    b2::DevBuf<uint32_t> ml_region, ml_clabels, ml_clidx, ml_csize, ml_cadj_ptr, ml_cadj_idx, ml_cdeg, ml_changed;
+    b2::DevBuf<uint64_t> ml_cptr, ml_cnt64;
+    b2::DevBuf<uint4> ml_cadj4;
+    b2::DevBuf<uint16_t> ml_cview;
+    b2::DevBuf<float> ml_ccost, ml_cwgt;
+    b2::DevBuf<uint32_t> ml_u32[3];
+    b2::DevBuf<uint64_t> ml_key[2];
+    b2::DevBuf<float> ml_f32;
+    uint32_t ml_nodes = 0;
     uint32_t *mrf_host_flags = nullptr;   // pinned: stop flags the host polls behind the launches it queued
     unsigned long long mrf_forest_nodes = 0, mrf_forest_nnz = 0;   // summed over the iterations of the last run
     uint32_t mrf_slow_trees = 0;
@@ -309,6 +321,10 @@ int mrf_prepare(b2tex_ctx *c, const b2tex_mrf_params *p);
 int mrf_energy_only(b2tex_ctx *c, int64_t *energy_fixed);
 int mrf_sample_only(b2tex_ctx *c, const b2tex_mrf_params *p, uint32_t t, uint32_t *level_host);
 int mrf_energy_double(b2tex_ctx *c, double *e, uint64_t *unseen);
+// multilevel view selection (mrf_multilevel.cu): contract c->labels into the ml_* buffers; project the coarse labels
+// back onto c->labels / c->mrf_lidx (a no-op once *stop != 0)
+int mrf_contract(b2tex_ctx *c, uint32_t *num_nodes);
+int mrf_project(b2tex_ctx *c, const uint32_t *stop);
 int seam_run(b2tex_ctx *c, b2tex_seam_info *info, bool solve = true);
 int seam_mg_export(b2tex_ctx *c, uint32_t rank, uint32_t nranks, void *handle64);
 int seam_mg_import(b2tex_ctx *c, uint32_t peer_rank, const void *handle64);

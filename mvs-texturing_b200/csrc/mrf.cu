@@ -22,6 +22,9 @@
 //   k_energy   fixed-point energy -> efix[t] on the device
 //   k_stop     StopWhenReturnsDiminish (view_selection.cpp:84) on the device; once it fires, the
 //              launches the host has already queued return immediately
+// use_multilevel (oracle/mrf_multilevel.c): after the stop rule fires, mrf_multilevel.cu contracts every same-label region
+// into one node and the same launches run on the contracted MRF with weighted Potts terms (k_tree<G, MINB, true>), each
+// iteration projected back onto the faces before k_energy (run_multilevel).
 #include <cooperative_groups.h>
 #include <stdlib.h>
 #include <string.h>
@@ -87,6 +90,7 @@ struct Mrf {
     uint16_t *J;                 // [3][mstride] position of that label in the child's list if the child should copy it, else 0xFFFF
     size_t mstride;
     uint32_t tree_cap;           // longest label list the shared-memory scratch of k_tree holds
+    const float *wgt;            // Potts weight per adjacency slot (the contracted MRF of mrf_multilevel.cu), read by k_tree<.., true>
 };
 // control block layout (uint32 words)
 constexpr int CTL_QN = 0;                        // [MAX_LEVELS+1] frontier sizes per round
@@ -589,7 +593,16 @@ __device__ __forceinline__ uint32_t level_run_end(LevPtr lev, uint32_t s, uint32
     return e;
 }
 
+// Potts weight of adjacency slot q of node v: 1 on the face graph, the number of fine edges on a contracted graph
+template <bool W>
+__device__ __forceinline__ float slot_weight(const Mrf &m, uint32_t v, uint32_t q)
+{
+    if constexpr (W) return m.wgt[m.adj_ptr[v] + q];
+    else return 1.0f;
+}
+
 // the same recursion through global memory: any degree, any size (one node at a time, 32 lanes over its labels)
+template <bool W>
 __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, uint32_t lane)
 {
     const uint16_t *lev = m.olev + start;
@@ -599,6 +612,14 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
             const uint32_t v = m.order[start + i];
             const uint64_t p0 = m.ptr[v], p1 = m.ptr[v + 1];
             const Nb nb = load_nb(m, v);
+            float wpar = 1.0f;   // weight of the edge to the parent
+            if constexpr (W) {
+                for (uint32_t q = 0; q < nb.deg; ++q) {
+                    const uint32_t w = nb_at(m, nb, q);
+                    const uint32_t pw = m.pos[w];
+                    if (m.labels[w] != 0 && pw != NO_NODE && pw < start + i) wpar = slot_weight<W>(m, v, q);
+                }
+            }
             float bh = INFINITY;
             uint32_t bk = 0xFFFFFFFFu;
             for (uint64_t k = p0 + lane; k < p1; k += 32) {
@@ -617,7 +638,7 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
                             h = h + msg;
                         }
                     } else {
-                        h = h + (lab != x ? 1.0f : 0.0f);
+                        h = h + (lab != x ? slot_weight<W>(m, v, q) : 0.0f);
                     }
                 }
                 m.H[k] = h;
@@ -628,7 +649,7 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
                 const uint32_t ok = __shfl_xor_sync(0xffffffffu, bk, sft);
                 if (oh < bh || (oh == bh && ok < bk)) { bh = oh; bk = ok; }
             }
-            if (lane == 0) { m.hminp1[v] = bh + 1.0f; m.amin[v] = bk; }
+            if (lane == 0) { m.hminp1[v] = bh + wpar; m.amin[v] = bk; }
         }
         __syncwarp();
         end = s;
@@ -662,7 +683,8 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
 // label bitmask [mw] u32 | prefix popcounts [mw] u16 (padded to 4 bytes)
 __host__ __device__ __forceinline__ uint32_t tree_group_bytes(uint32_t cap, uint32_t mw) { return cap * 6u + mw * 4u + ((mw * 2u + 3u) & ~3u); }
 
-template <int G, int MINB>
+// W: weighted Potts terms (slot_weight); the unweighted instantiation is the face-graph solver
+template <int G, int MINB, bool W = false>
 __global__ void __launch_bounds__(TREE_THREADS, MINB) k_tree(Mrf m)
 {
     if (__ldcg(m.state + ST_STOP)) return;
@@ -690,7 +712,7 @@ __global__ void __launch_bounds__(TREE_THREADS, MINB) k_tree(Mrf m)
         const uint32_t cnt = te.x & 0x7FFFFFFFu, start = te.z;
         if (te.x >> 31) {   // a node of degree > 3 or a label list longer than the scratch
             if (lane == 0) atomicAdd(m.state + ST_SLOW, 1u);
-            tree_solve_global(m, start, cnt, lane);
+            tree_solve_global<W>(m, start, cnt, lane);
             continue;
         }
         NodeRec *rec = m.rec + start;
@@ -726,6 +748,15 @@ __global__ void __launch_bounds__(TREE_THREADS, MINB) k_tree(Mrf m)
             const uint32_t ps = r1.w & 3u, pn = has_parent ? (r1.w >> 16) : 0u;
             const uint64_t pp0 = ((uint64_t)r2.y << 32) | r2.x;
             const uint16_t *pview = m.view + pp0;
+            float w0 = 1.0f, w1 = 1.0f, w2 = 1.0f;   // Potts weights of the three slots
+            if constexpr (W) {
+                if (act) {
+                    const float *wr = m.wgt + m.adj_ptr[r0.x];
+                    if (e0 & NBR_KIND) w0 = wr[0];
+                    if (e1 & NBR_KIND) w1 = wr[1];
+                    if (e2 & NBR_KIND) w2 = wr[2];
+                }
+            }
             // the parent's labels this lane will look up: loaded together with the node's own rows, not after the reduction
             uint32_t want[PRE];
 #pragma unroll
@@ -742,9 +773,9 @@ __global__ void __launch_bounds__(TREE_THREADS, MINB) k_tree(Mrf m)
                 const uint32_t vw = viewv[k];
                 const uint32_t lab = vw + 1u;
                 float h = costv[k];
-                if (c0) h = h + __ldcg(m0 + k); else if (x0) h = h + (lab != x0 ? 1.0f : 0.0f);
-                if (c1) h = h + __ldcg(m1 + k); else if (x1) h = h + (lab != x1 ? 1.0f : 0.0f);
-                if (c2) h = h + __ldcg(m2 + k); else if (x2) h = h + (lab != x2 ? 1.0f : 0.0f);
+                if (c0) h = h + __ldcg(m0 + k); else if (x0) h = h + (lab != x0 ? w0 : 0.0f);
+                if (c1) h = h + __ldcg(m1 + k); else if (x1) h = h + (lab != x1 ? w1 : 0.0f);
+                if (c2) h = h + __ldcg(m2 + k); else if (x2) h = h + (lab != x2 ? w2 : 0.0f);
                 Hs[k] = h;
                 if (mw) atomicOr(Ms + (vw >> 5), 1u << (vw & 31u)); else Vs[k] = (uint16_t)vw;
                 if (h < bh) { bh = h; bk = k; }
@@ -756,7 +787,7 @@ __global__ void __launch_bounds__(TREE_THREADS, MINB) k_tree(Mrf m)
                 bk = __reduce_min_sync(gmask, hb == hmin ? bk : 0xFFFFFFFFu);
                 bh = __uint_as_float(hmin);
             }
-            const float hm = bh + 1.0f;
+            const float hm = bh + ((e0 & NBR_KIND) == NBR_PARENT ? w0 : (e1 & NBR_KIND) == NBR_PARENT ? w1 : w2);   // + weight to the parent
             __syncwarp();
             if (act && glane == 0) {   // for the top-down pass: the best label given the subtree, position and value
                 rec[i].amin = bk;
@@ -1047,6 +1078,25 @@ Mrf make_mrf(b2tex_ctx *c, uint32_t iter)
     m.rec = reinterpret_cast<NodeRec *>(c->mrf_rec.p);
     m.M = c->mrf_M.p; m.J = c->mrf_J.p; m.mstride = c->nnz;
     m.tree_cap = c->mrf_tree_cap;
+    m.wgt = nullptr;
+    return m;
+}
+
+// The contracted MRF of mrf_contract (single GPU, whole mesh) with the fine run's scratch, seed and iteration numbers.  The
+// push stamps stay where make_mrf put them (queue + 2 F, beyond both frontier lists of the n <= F coarse nodes): a stamp is
+// unique per (iteration, round), and iteration numbers go on from the fine phases.
+Mrf make_coarse_mrf(b2tex_ctx *c, uint32_t iter)
+{
+    Mrf m = make_mrf(c, iter);
+    const uint32_t n = c->ml_nodes;
+    m.F = n; m.nb = 0; m.ne = n;
+    m.adj_ptr = c->ml_cadj_ptr.p; m.adj_idx = c->ml_cadj_idx.p; m.adj4 = c->ml_cadj4.p; m.wgt = c->ml_cwgt.p;
+    m.ptr = c->ml_cptr.p; m.view = c->ml_cview.p; m.cost = c->ml_ccost.p;
+    m.labels = c->ml_clabels.p; m.lidx = c->ml_clidx.p;
+    m.part_size = n ? n : 1;
+    const uint32_t rd = c->mrf_params.root_div;
+    if (rd == 0) m.rdiv = 0;
+    else { uint32_t cap = n / 8u; if (cap < 1u) cap = 1u; m.rdiv = rd < cap ? rd : cap; }
     return m;
 }
 
@@ -1078,24 +1128,24 @@ int launch_forest(b2tex_ctx *c, Mrf &m, int build_trees)
     return B2TEX_OK;
 }
 
-template <int G, int MINB>
+template <int G, int MINB, bool W>
 int launch_tree_variant(b2tex_ctx *c, Mrf &m)
 {
     static bool attr_set = false;   // opt in to > 48 KB of dynamic shared memory (per function, once)
     if (!attr_set) {
-        B2_CUDA(cudaFuncSetAttribute(k_tree<G, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        B2_CUDA(cudaFuncSetAttribute(k_tree<G, MINB, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         attr_set = true;
     }
     int per_sm = 0;
-    B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_tree<G, MINB>, TREE_THREADS, m.tree_smem));
+    B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_tree<G, MINB, W>, TREE_THREADS, m.tree_smem));
     if (per_sm < 1) { set_error("k_tree cannot be resident with %u bytes of shared memory", m.tree_smem); return B2TEX_ERR_CUDA; }
     const int grid = c->num_sms * per_sm;
-    B2_LAUNCH k_tree<G, MINB><<<grid, TREE_THREADS, m.tree_smem, c->stream>>>(m);
+    B2_LAUNCH k_tree<G, MINB, W><<<grid, TREE_THREADS, m.tree_smem, c->stream>>>(m);
     B2_KERNEL_CHECK();
     return B2TEX_OK;
 }
 
-template <int G>
+template <int G, bool W = false>
 int launch_tree(b2tex_ctx *c, Mrf &m)
 {
     const uint32_t n = m.ne - m.nb;
@@ -1103,7 +1153,7 @@ int launch_tree(b2tex_ctx *c, Mrf &m)
     // 2 CTAs of 512 threads per SM (64 registers) or 3 (40 registers, a few spills): the kernel lives on resident warps, but
     // on an H100 SXM (700 W) the spill-free variant is faster (C3: k_tree 28.7 against 44.6 ms per pass)
     static const int minb = getenv("B2TEX_TREE_BLOCKS") ? atoi(getenv("B2TEX_TREE_BLOCKS")) : 2;
-    return minb == 3 ? launch_tree_variant<G, 3>(c, m) : launch_tree_variant<G, 2>(c, m);
+    return minb == 3 ? launch_tree_variant<G, 3, W>(c, m) : launch_tree_variant<G, 2, W>(c, m);
 }
 
 // peers of this context, or nranks == 1
@@ -1136,8 +1186,9 @@ int launch_energy(b2tex_ctx *c, Mrf &m, uint32_t t)
     return B2TEX_OK;
 }
 
-// label halo -> barrier -> partial energies -> barrier + all-reduce + stop rule (multi-GPU), or energy + stop rule
-int enqueue_exchange_and_energy(b2tex_ctx *c, Mrf &m, uint32_t t, bool stop_rule)
+// label halo -> barrier -> partial energies -> barrier + all-reduce + stop rule (multi-GPU), or energy + stop rule.
+// t_ref: the iteration the stop rule's window restarts from (a phase of multilevel view selection, single GPU only)
+int enqueue_exchange_and_energy(b2tex_ctx *c, Mrf &m, uint32_t t, bool stop_rule, uint32_t t_ref = 0)
 {
     cudaStream_t s = c->stream;
     const b2tex_mrf_params &p = c->mrf_params;
@@ -1147,7 +1198,11 @@ int enqueue_exchange_and_energy(b2tex_ctx *c, Mrf &m, uint32_t t, bool stop_rule
             ScopedTimer te(c, "mrf.k_energy", 12.0 * (double)(m.ne - m.nb));
             B2_TRY(launch_energy(c, m, t));
         }
-        if (stop_rule) B2_LAUNCH k_stop<<<1, 1, 0, s>>>(m, t, window, p.ratio, p.max_iterations);
+        if (stop_rule) {   // k_stop on the phase's own iteration numbers: ST_STOP / ST_DONE are relative to t_ref
+            Mrf ms = m;
+            ms.efix = m.efix + t_ref;
+            B2_LAUNCH k_stop<<<1, 1, 0, s>>>(ms, t - t_ref, window, p.ratio, p.max_iterations - t_ref);
+        }
         B2_KERNEL_CHECK();
         return B2TEX_OK;
     }
@@ -1169,7 +1224,7 @@ int enqueue_exchange_and_energy(b2tex_ctx *c, Mrf &m, uint32_t t, bool stop_rule
     return B2TEX_OK;
 }
 
-int enqueue_iteration(b2tex_ctx *c, Mrf &m, bool stop_rule)
+int enqueue_iteration(b2tex_ctx *c, Mrf &m, bool stop_rule, uint32_t t_ref = 0)
 {
     if (m.ne <= m.nb && !mg_active(c)) return B2TEX_OK;
     {
@@ -1185,7 +1240,33 @@ int enqueue_iteration(b2tex_ctx *c, Mrf &m, bool stop_rule)
             default: B2_TRY(launch_tree<32>(c, m)); break;
         }
     }
-    return enqueue_exchange_and_energy(c, m, m.iter, stop_rule);
+    return enqueue_exchange_and_energy(c, m, m.iter, stop_rule, t_ref);
+}
+
+// one iteration of the BCD on the contracted MRF (weighted Potts terms), the projection onto the faces, and the fine
+// energy + stop rule (window restarted at t_ref)
+int enqueue_coarse_iteration(b2tex_ctx *c, uint32_t t, uint32_t t_ref)
+{
+    Mrf cm = make_coarse_mrf(c, t);
+    {
+        ScopedTimer tf(c, "mrf.k_forest");
+        B2_TRY(launch_forest(c, cm, 1));
+    }
+    {
+        ScopedTimer tu(c, "mrf.k_tree_weighted");
+        switch (c->mrf_group) {
+            case 4: B2_TRY((launch_tree<4, true>(c, cm))); break;
+            case 8: B2_TRY((launch_tree<8, true>(c, cm))); break;
+            case 16: B2_TRY((launch_tree<16, true>(c, cm))); break;
+            default: B2_TRY((launch_tree<32, true>(c, cm))); break;
+        }
+    }
+    Mrf m = make_mrf(c, t);
+    {
+        ScopedTimer tp(c, "mrf_ml.project");
+        B2_TRY(mrf_project(c, m.state + ST_STOP));
+    }
+    return enqueue_exchange_and_energy(c, m, t, true, t_ref);
 }
 
 int alloc_mrf(b2tex_ctx *c, const b2tex_mrf_params *p)
@@ -1355,11 +1436,102 @@ int mrf_iterate(b2tex_ctx *c, uint32_t t, int64_t *efix)
     return B2TEX_OK;
 }
 
-// The whole run without a host round trip per iteration: the host queues iterations ahead of the device; the stop rule
-// is evaluated on the device and turns the launches that are already queued behind it into no-ops.  With peers attached
-// (mrf_mg_export / mrf_mg_import) every rank runs this same loop; the ranks meet inside the kernels.
+// Iterations t_begin .. max_iterations (fine, or on the contracted MRF) without a host round trip per iteration: the host
+// queues iterations ahead of the device; the stop rule is evaluated on the device and turns the launches that are already
+// queued behind it into no-ops.  With peers attached (mrf_mg_export / mrf_mg_import) every rank runs this same loop; the
+// ranks meet inside the kernels.
+int run_phase(b2tex_ctx *c, uint32_t t_begin, uint32_t t_ref, bool coarse)
+{
+    cudaStream_t s = c->stream;
+    const uint32_t max_it = c->mrf_params.max_iterations;
+    constexpr int LAG = 3;   // iterations queued beyond the last one whose stop flag the host has seen
+    cudaEvent_t ev[LAG + 1];
+    for (auto &e : ev) B2_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    volatile uint32_t *hf = c->mrf_host_flags;
+    int rc = B2TEX_OK;
+    for (uint32_t t = t_begin; t <= max_it; ++t) {
+        Mrf m = make_mrf(c, t);
+        rc = coarse ? enqueue_coarse_iteration(c, t, t_ref) : enqueue_iteration(c, m, true, t_ref);
+        if (rc != B2TEX_OK) break;
+        const int slot = (int)(t % (LAG + 1));
+        if (cudaMemcpyAsync((void *)&hf[slot], m.state + ST_STOP, 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+            cudaEventRecord(ev[slot], s) != cudaSuccess) {
+            set_error("view selection: %s", cudaGetErrorString(cudaGetLastError()));
+            rc = B2TEX_ERR_CUDA;
+            break;
+        }
+        if (t - t_begin >= (uint32_t)LAG) {
+            const int w = (int)((t - LAG) % (LAG + 1));
+            if (cudaEventSynchronize(ev[w]) != cudaSuccess) { set_error("view selection: %s", cudaGetErrorString(cudaGetLastError())); rc = B2TEX_ERR_CUDA; break; }
+            if (hf[w]) break;   // the rule fired LAG iterations ago; what is queued behind it returns at once
+        }
+    }
+    if (cudaStreamSynchronize(s) != cudaSuccess && rc == B2TEX_OK) {
+        set_error("view selection: %s", cudaGetErrorString(cudaGetLastError()));
+        rc = B2TEX_ERR_CUDA;
+    }
+    for (auto &e : ev) cudaEventDestroy(e);
+    return rc;
+}
+
+// last iteration of the phase that started after t_ref
+int phase_end(b2tex_ctx *c, uint32_t t_ref, uint32_t *t_end)
+{
+    uint32_t st[2];
+    B2_CUDA(cudaMemcpyAsync(st, c->mrf_state.p + ST_STOP, sizeof(st), cudaMemcpyDeviceToHost, c->stream));
+    B2_CUDA(cudaStreamSynchronize(c->stream));
+    static_assert(ST_DONE == ST_STOP + 1, "state layout");
+    *t_end = t_ref + (st[0] ? st[0] : st[1]);
+    return B2TEX_OK;
+}
+
+// The multilevel schedule of oracle/mrf_multilevel.c, after the first fine phase: contract the labeling, run the BCD on
+// the contracted MRF from the current labels (every iteration projected, the trace and the stop rule on fine energies,
+// window restarted), and go back to a fine phase while the coarse phase strictly lowered the energy.
+int run_multilevel(b2tex_ctx *c, b2tex_mrf_info *info, uint32_t *t_ref)
+{
+    const uint32_t max_it = c->mrf_params.max_iterations;
+    const Mrf m = make_mrf(c, 0);
+    uint32_t t = 0;
+    B2_TRY(phase_end(c, 0, &t));
+    while (t < max_it) {
+        int64_t before = 0, after = 0;
+        B2_TRY(read_energy(c, m, t, &before));
+        uint32_t n = 0;
+        {
+            ScopedTimer tc(c, "mrf_ml.contract");
+            B2_TRY(mrf_contract(c, &n));
+            if (n) B2_LAUNCH k_build_adj4<<<(n + 255) / 256, 256, 0, c->stream>>>(n, c->ml_cadj_ptr.p, c->ml_cadj_idx.p, c->ml_cadj4.p);
+            B2_KERNEL_CHECK();
+        }
+        info->coarse_nodes = n;
+        B2_CUDA(cudaMemsetAsync(m.state + ST_STOP, 0, sizeof(uint32_t), c->stream));
+        B2_TRY(run_phase(c, t + 1, t, true));
+        *t_ref = t;
+        uint32_t t2 = 0;
+        B2_TRY(phase_end(c, t, &t2));
+        B2_TRY(read_energy(c, m, t2, &after));
+        if (!(after < before)) break;
+        info->multilevel_passes++;
+        if (t2 >= max_it) break;
+        B2_CUDA(cudaMemsetAsync(m.state + ST_STOP, 0, sizeof(uint32_t), c->stream));
+        B2_TRY(run_phase(c, t2 + 1, t2, false));
+        *t_ref = t2;
+        B2_TRY(phase_end(c, t2, &t));
+    }
+    return B2TEX_OK;
+}
+
+// The whole run: init, the iterations (run_phase), and with use_multilevel the multilevel schedule (run_multilevel).
 int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, double *trace)
 {
+    info->multilevel_passes = 0;
+    info->coarse_nodes = 0;
+    if (p->use_multilevel && ((p->num_parts ? p->num_parts : 1) > 1 || mg_active(c) || c->face_begin != 0 || c->face_end != c->F)) {
+        set_error("multilevel view selection: one GPU and the whole mesh only (num_parts %u, %s, face range %u..%u of %u)",
+                  p->num_parts, mg_active(c) ? "peers attached" : "no peers", c->face_begin, c->face_end, c->F);
+        return B2TEX_ERR_UNSUPPORTED;
+    }
     int64_t e0 = 0;
     B2_TRY(mrf_init(c, p, &e0));
     cudaStream_t s = c->stream;
@@ -1374,34 +1546,9 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
         return B2TEX_OK;
     }
     invalidate(c, LABELS);   // until the iterations below have finished without error
-    constexpr int LAG = 3;   // iterations queued beyond the last one whose stop flag the host has seen
-    cudaEvent_t ev[LAG + 1];
-    for (auto &e : ev) B2_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    volatile uint32_t *hf = c->mrf_host_flags;
-    int rc = B2TEX_OK;
-    for (uint32_t t = 1; t <= max_it; ++t) {
-        Mrf m = make_mrf(c, t);
-        rc = enqueue_iteration(c, m, true);
-        if (rc != B2TEX_OK) break;
-        const int slot = (int)(t % (LAG + 1));
-        if (cudaMemcpyAsync((void *)&hf[slot], m.state + ST_STOP, 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-            cudaEventRecord(ev[slot], s) != cudaSuccess) {
-            set_error("view selection: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = B2TEX_ERR_CUDA;
-            break;
-        }
-        if (t > (uint32_t)LAG) {
-            const int w = (int)((t - LAG) % (LAG + 1));
-            if (cudaEventSynchronize(ev[w]) != cudaSuccess) { set_error("view selection: %s", cudaGetErrorString(cudaGetLastError())); rc = B2TEX_ERR_CUDA; break; }
-            if (hf[w]) break;   // the rule fired LAG iterations ago; what is queued behind it returns at once
-        }
-    }
-    if (cudaStreamSynchronize(s) != cudaSuccess && rc == B2TEX_OK) {
-        set_error("view selection: %s", cudaGetErrorString(cudaGetLastError()));
-        rc = B2TEX_ERR_CUDA;
-    }
-    for (auto &e : ev) cudaEventDestroy(e);
-    B2_TRY(rc);
+    B2_TRY(run_phase(c, 1, 0, false));
+    uint32_t t_ref = 0;   // the stop rule's reference iteration of the last phase: ST_STOP / ST_DONE count from it
+    if (p->use_multilevel) B2_TRY(run_multilevel(c, info, &t_ref));
     Mrf m = make_mrf(c, 0);
     if (mg) {   // one all-gather of the final labels by peer stores: seam leveling assembles its system on every rank
         MrfPeers pr = make_peers(c);
@@ -1425,7 +1572,7 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
         memcpy(efix.data(), pin_e, ((size_t)max_it + 1) * sizeof(unsigned long long));
     }
     if (st[ST_ERR]) { set_error("multi-GPU view selection: %u cross-GPU barrier timeouts (a peer did not arrive)", st[ST_ERR]); return B2TEX_ERR_CUDA; }
-    const uint32_t t_end = st[ST_STOP] ? st[ST_STOP] : st[ST_DONE];   // ST_STOP == 0 only for max_iterations == 0
+    const uint32_t t_end = t_ref + (st[ST_STOP] ? st[ST_STOP] : st[ST_DONE]);   // ST_STOP == 0 only for max_iterations == 0
     info->iterations = t_end;
     info->energy_initial = (double)(int64_t)efix[0] / 4294967296.0;
     info->energy_final = (double)(int64_t)efix[t_end] / 4294967296.0;
