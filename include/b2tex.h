@@ -75,6 +75,13 @@ typedef struct {
                                   region into one node, solve the contracted MRF (weighted Potts) from the current labels
                                   and go back to the faces while that lowers the energy.  One GPU, whole mesh, num_parts 1
                                   only (else B2TEX_ERR_UNSUPPORTED).  Default 0. */
+    uint32_t use_spanning_tree;   /* mapMAP_control::use_spanning_tree: before the iterations on induced forests, a phase of
+                                     iterations on spanning forests of the seen faces (BFS from the same roots, every
+                                     non-tree neighbour fixed at its label from the start of the iteration; an iteration
+                                     that raises the energy is undone), until the stop rule fires.  The induced-forest
+                                     phase follows with the window restarted, then the multilevel schedule if
+                                     use_multilevel.  One GPU, whole mesh, num_parts 1 only (else B2TEX_ERR_UNSUPPORTED).
+                                     Default 0. */
 } b2tex_mrf_params;
 
 typedef struct {
@@ -85,6 +92,8 @@ typedef struct {
     uint64_t sweep_bytes;  /* algorithmic bytes of one sweep (SURVEY 8d): 14 nnz + 20 F */
     uint32_t multilevel_passes;   /* use_multilevel: contractions whose coarse solve lowered the energy */
     uint32_t coarse_nodes;        /* use_multilevel: nodes of the last contraction */
+    uint32_t spanning_tree_iterations;   /* use_spanning_tree: iterations of the spanning phase (numbered 1 ..) */
+    uint32_t spanning_tree_rejected;     /* use_spanning_tree: of those, the ones that were undone */
 } b2tex_mrf_info;
 
 typedef struct {

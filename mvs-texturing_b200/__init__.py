@@ -60,13 +60,15 @@ class B2DcInfo(C.Structure):
 class B2MrfParams(C.Structure):
     _fields_ = [("max_iterations", C.c_uint32), ("rounds", C.c_uint32), ("root_div", C.c_uint32),
                 ("seed", C.c_uint32), ("window", C.c_uint32), ("ratio", C.c_float),
-                ("num_parts", C.c_uint32), ("num_views", C.c_uint32), ("use_multilevel", C.c_uint32)]
+                ("num_parts", C.c_uint32), ("num_views", C.c_uint32), ("use_multilevel", C.c_uint32),
+                ("use_spanning_tree", C.c_uint32)]
 
 
 class B2MrfInfo(C.Structure):
     _fields_ = [("iterations", C.c_uint32), ("energy_initial", C.c_double),
                 ("energy_final", C.c_double), ("unseen", C.c_uint64), ("sweep_bytes", C.c_uint64),
-                ("multilevel_passes", C.c_uint32), ("coarse_nodes", C.c_uint32)]
+                ("multilevel_passes", C.c_uint32), ("coarse_nodes", C.c_uint32),
+                ("spanning_tree_iterations", C.c_uint32), ("spanning_tree_rejected", C.c_uint32)]
 
 
 class B2PatchInfo(C.Structure):

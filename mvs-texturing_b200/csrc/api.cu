@@ -39,6 +39,7 @@ void b2tex_default_mrf_params(b2tex_mrf_params *p)
     p->num_parts = 1;
     p->num_views = 0;
     p->use_multilevel = 0;
+    p->use_spanning_tree = 0;
 }
 
 int b2tex_create(int device, b2tex_ctx **out)

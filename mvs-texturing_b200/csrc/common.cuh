@@ -217,6 +217,9 @@ struct b2tex_ctx {
     b2::DevBuf<uint4> mrf_rec;         // [3 F] 48-byte node records in forest order (k_tree_prep)
     b2::DevBuf<uint4> mrf_adj4;        // compact degree<=3 adjacency
     b2::DevBuf<uint32_t> mrf_queue;    // forest frontier lists + stamps
+    b2::DevBuf<uint32_t> mrf_par;      // spanning-tree view selection only: parent of every node in the spanning forest
+    b2::DevBuf<uint32_t> mrf_snap;     // spanning-tree view selection only: [2][F] labels and label positions at the start
+                                       // of an iteration
     // the contracted MRF of multilevel view selection (mrf_multilevel.cu), grow-only scratch: node of every face, per node
     // label / label position / size / label-list offsets / CSR row / compact adjacency, coarse label lists and edges, and the
     // sort and scan buffers of the contraction (max(nnz, adjacency entries) each)

@@ -25,6 +25,10 @@
 // use_multilevel (oracle/mrf_multilevel.c): after the stop rule fires, mrf_multilevel.cu contracts every same-label region
 // into one node and the same launches run on the contracted MRF with weighted Potts terms (k_tree<G, MINB, true>), each
 // iteration projected back onto the faces before k_energy (run_multilevel).
+// use_spanning_tree (oracle/mrf_spanning.c): a spanning phase before the first acyclic one.  k_forest<true> grows a BFS
+// spanning forest from the same roots and records every node's parent in `par`; k_tree_prep<true> classifies neighbours by
+// `par` (every non-tree neighbour is fixed at its label from the start of the iteration), and k_accept / k_restore undo an
+// iteration that raised the energy.
 #include <cooperative_groups.h>
 #include <stdlib.h>
 #include <string.h>
@@ -91,12 +95,15 @@ struct Mrf {
     size_t mstride;
     uint32_t tree_cap;           // longest label list the shared-memory scratch of k_tree holds
     const float *wgt;            // Potts weight per adjacency slot (the contracted MRF of mrf_multilevel.cu), read by k_tree<.., true>
+    uint32_t *par;               // spanning forests: parent of every node, NO_NODE for roots and nodes outside the forest
+    uint32_t *snap, *snap_lidx;  // spanning forests: labels and label positions at the start of the iteration
 };
 // control block layout (uint32 words)
 constexpr int CTL_QN = 0;                        // [MAX_LEVELS+1] frontier sizes per round
 constexpr int CTL_NROOTS = MAX_LEVELS + 8;       // trees of this iteration
 constexpr int CTL_CURSOR = MAX_LEVELS + 9;       // forest nodes laid out so far
 constexpr int CTL_CLAIM = MAX_LEVELS + 10;       // k_tree: next unclaimed tree
+constexpr int CTL_REJECT = MAX_LEVELS + 11;      // spanning iteration: k_accept rejected it, k_restore brings the labels back
 constexpr int CTL_MAXPRIO = MAX_LEVELS + 12;     // 64-bit, 8-byte aligned
 constexpr int CTL_WORDS = MAX_LEVELS + 32;
 // run state (uint32 words)
@@ -108,6 +115,7 @@ constexpr int ST_FNODES = 4;    // 64-bit: forest nodes summed over the iteratio
 constexpr int ST_FNNZ = 6;      // 64-bit: labels of forest nodes summed over the iterations
 constexpr int ST_SLOW = 8;      // trees that went through global memory
 constexpr int ST_ERR = 9;       // cross-GPU barrier timeouts (a peer did not arrive)
+constexpr int ST_REJECTED = 10; // spanning iterations that raised the energy and were undone
 constexpr int ST_WORDS = 16;
 
 __device__ __forceinline__ bool same_part(const Mrf &m, uint32_t a, uint32_t b)
@@ -225,6 +233,13 @@ __device__ __forceinline__ uint32_t count_in_forest(const Mrf &m, uint32_t v, ui
 }
 
 constexpr int FOREST_THREADS = 1024;
+// growth rounds at most: `rounds` for induced forests, the bound alloc_mrf puts on `rounds` for spanning forests
+template <bool S>
+__device__ __forceinline__ uint32_t growth_rounds(const Mrf &m) { return S ? (uint32_t)(MAX_LEVELS - 2) : m.rounds; }
+// S: spanning forest (oracle/mrf_spanning.c) -- every queued undecided node joins, under its strongest neighbour of the
+// previous level (recorded in m.par), until a round adds nobody or after MAX_LEVELS - 2 rounds; round 0 also snapshots the
+// labels for k_restore
+template <bool S = false>
 __global__ void __launch_bounds__(FOREST_THREADS, 1) k_forest(Mrf m, int build_trees)
 {
     cg::grid_group grid = cg::this_grid();
@@ -279,6 +294,9 @@ __global__ void __launch_bounds__(FOREST_THREADS, 1) k_forest(Mrf m, int build_t
             lvl = !eligible ? LVL_DEAD : (is_root ? 0u : LVL_NONE);
         }
         if (valid) { m.level[v] = lvl; if (build_trees) m.pos[v] = NO_NODE; }
+        if constexpr (S) {
+            if (valid) { m.par[v] = NO_NODE; m.snap[v] = m.labels[v]; m.snap_lidx[v] = m.lidx[v]; }
+        }
         if (build_trees) {
             const bool is_root = valid && lvl == 0u;
             if (threadIdx.x == 0) s_cnt = 0;
@@ -339,8 +357,11 @@ __global__ void __launch_bounds__(FOREST_THREADS, 1) k_forest(Mrf m, int build_t
     }
     grid.sync();
     stamp(2);   // frontier seeding
-    for (uint32_t r = 1; r <= m.rounds; ++r) {
+    for (uint32_t r = 1; r <= growth_rounds<S>(m); ++r) {
         const uint32_t n = __ldcg(m.ctl + CTL_QN + r);
+        if constexpr (S) {
+            if (n == 0) break;   // final since the last grid.sync(): grid-uniform
+        }
         const uint32_t *q = m.queue + (size_t)(r & 1u) * m.F;
         for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += nth) {   // block-uniform trip count
             const uint32_t qi = base + threadIdx.x;
@@ -349,7 +370,16 @@ __global__ void __launch_bounds__(FOREST_THREADS, 1) k_forest(Mrf m, int build_t
                 const Nb nb = load_nb(m, v);
                 uint32_t c = 0, parent = NO_NODE;
                 bool win = true;
-                if (nb.deg <= 3) {
+                if constexpr (S) {   // a queued node has a neighbour of level r - 1 (and none lower): it joins
+                    uint32_t pp = 0;
+                    for (uint32_t i = 0; i < nb.deg; ++i) {
+                        const uint32_t w = nb_at(m, nb, i);
+                        if (!local_pair(m, v, w) || __ldcg(m.level + w) >= r) continue;
+                        const uint32_t pw = prio(w, seed_t);
+                        if (parent == NO_NODE || pw > pp) { parent = w; pp = pw; }
+                    }
+                    c = parent != NO_NODE ? 1u : 0u;
+                } else if (nb.deg <= 3) {
                     // manifold degree: every load of a hop is issued before the first one is used (the round is a chain of
                     // dependent loads; two hops instead of up to eight round trips)
                     const uint32_t wn[3] = {nb.x, nb.y, nb.z};
@@ -409,6 +439,7 @@ __global__ void __launch_bounds__(FOREST_THREADS, 1) k_forest(Mrf m, int build_t
                 else if (c == 1) {
                     if (win) {
                         m.level[v] = r;
+                        if constexpr (S) m.par[v] = parent;
                         if (build_trees) {   // the parent joined in an earlier round: its (tree, slot) is final
                             const uint2 pj = __ldcg(m.tjoin + parent);
                             uint4 *te = m.ttab + pj.x;
@@ -418,17 +449,17 @@ __global__ void __launch_bounds__(FOREST_THREADS, 1) k_forest(Mrf m, int build_t
                             if (nb.deg > 3) atomicOr(&te->x, 0x80000000u);
                             m.tjoin[v] = make_uint2(pj.x, slot);
                         }
-                        if (r < m.rounds)
+                        if (r < growth_rounds<S>(m))
                             for (uint32_t i = 0; i < nb.deg; ++i) {
                                 uint32_t w = nb_at(m, nb, i);
                                 if (local_pair(m, v, w) && __ldcg(m.level + w) == LVL_NONE) push(w, r + 1u);
                             }
-                    } else if (r < m.rounds) {
+                    } else if (r < growth_rounds<S>(m)) {
                         push(v, r + 1u);
                     }
                 }
             }
-            if (r < m.rounds) flush(r + 1u);
+            if (r < growth_rounds<S>(m)) flush(r + 1u);
         }
         grid.sync();
     }
@@ -466,7 +497,7 @@ __global__ void __launch_bounds__(FOREST_THREADS, 1) k_forest(Mrf m, int build_t
     unsigned long long fn = 0, fz = 0;
     for (uint32_t v = m.nb + tid; v < m.ne; v += nth) {
         const uint32_t l = __ldcg(m.level + v);
-        if (l > m.rounds) continue;
+        if (l > growth_rounds<S>(m)) continue;
         const uint2 tj = __ldcg(m.tjoin + v);
         const uint32_t idx = __ldcg(&m.ttab[tj.x].z) + tj.y;
         m.order[idx] = v;
@@ -521,6 +552,9 @@ struct __align__(16) NodeRec {
 };
 static_assert(sizeof(NodeRec) == 48, "NodeRec layout");
 
+// S: spanning forest -- children are the neighbours w with par[w] == v, the parent is par[v], every other seen neighbour
+// is fixed at the label it has now (before k_tree writes any)
+template <bool S = false>
 __global__ void __launch_bounds__(256) k_tree_prep(Mrf m)
 {
     if (__ldcg(m.state + ST_STOP)) return;
@@ -541,12 +575,18 @@ __global__ void __launch_bounds__(256) k_tree_prep(Mrf m)
         uint32_t xl[3] = {0u, 0u, 0u}, pl[3] = {NO_NODE, NO_NODE, NO_NODE}, wn[3] = {a4.x, a4.y, a4.z};
 #pragma unroll
         for (int a = 0; a < 3; ++a)
-            if ((uint32_t)a < a4.w && wn[a] != NO_NODE) { xl[a] = m.labels[wn[a]]; pl[a] = m.pos[wn[a]]; }
+            if ((uint32_t)a < a4.w && wn[a] != NO_NODE) { xl[a] = m.labels[wn[a]]; pl[a] = S ? m.par[wn[a]] : m.pos[wn[a]]; }
+        const uint32_t pv = S ? m.par[v] : NO_NODE;
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
             if (xl[a] == 0u) continue;   // unseen faces carry no edges (view_selection.cpp:30,35)
-            if (pl[a] == NO_NODE) { r.nbr[a] = NBR_FIXED | xl[a]; continue; }
-            if (pl[a] > i) { r.nbr[a] = NBR_CHILD; continue; }   // a forest neighbour is in the same tree: deeper = child
+            if constexpr (S) {   // pl = the neighbour's parent
+                if (pl[a] == v) { r.nbr[a] = NBR_CHILD; continue; }
+                if (wn[a] != pv) { r.nbr[a] = NBR_FIXED | xl[a]; continue; }
+            } else {
+                if (pl[a] == NO_NODE) { r.nbr[a] = NBR_FIXED | xl[a]; continue; }
+                if (pl[a] > i) { r.nbr[a] = NBR_CHILD; continue; }   // a forest neighbour is in the same tree: deeper = child
+            }
             const uint32_t w = wn[a];
             const uint4 b4 = __ldg(m.adj4 + w);
             const uint64_t q0 = m.ptr[w];
@@ -601,8 +641,10 @@ __device__ __forceinline__ float slot_weight(const Mrf &m, uint32_t v, uint32_t 
     else return 1.0f;
 }
 
-// the same recursion through global memory: any degree, any size (one node at a time, 32 lanes over its labels)
-template <bool W>
+// the same recursion through global memory: any degree, any size (one node at a time, 32 lanes over its labels).
+// S: a spanning forest, classified by m.par as k_tree_prep<true> does; fixed labels come from the snapshot, because the
+// top-down passes of other warps write m.labels meanwhile and a spanning tree has edges to other trees.
+template <bool W, bool S = false>
 __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, uint32_t lane)
 {
     const uint16_t *lev = m.olev + start;
@@ -622,11 +664,25 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
             }
             float bh = INFINITY;
             uint32_t bk = 0xFFFFFFFFu;
+            const uint32_t par_v = S ? m.par[v] : NO_NODE;
             for (uint64_t k = p0 + lane; k < p1; k += 32) {
                 const uint32_t lab = (uint32_t)m.view[k] + 1u;
                 float h = m.cost[k];
                 for (uint32_t q = 0; q < nb.deg; ++q) {
                     const uint32_t w = nb_at(m, nb, q);
+                    if constexpr (S) {
+                        const uint32_t x = m.snap[w];
+                        if (x == 0) continue;
+                        if (__ldcg(m.par + w) == v) {   // child
+                            float msg = __ldcg(m.hminp1 + w);
+                            const long long j = find_label(m, w, lab);
+                            if (j >= 0) { const float hw = __ldcg(m.H + j); if (hw < msg) msg = hw; }
+                            h = h + msg;
+                        } else if (w != par_v) {
+                            h = h + (lab != x ? 1.0f : 0.0f);
+                        }
+                        continue;
+                    }
                     const uint32_t x = m.labels[w];
                     if (x == 0) continue;
                     const uint32_t pw = m.pos[w];
@@ -660,7 +716,14 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
             const uint32_t v = m.order[start + i];
             uint32_t bk = __ldcg(m.amin + v);
             const Nb nb = load_nb(m, v);
-            for (uint32_t q = 0; q < nb.deg; ++q) {
+            if constexpr (S) {
+                const uint32_t pv = m.par[v];
+                if (pv != NO_NODE) {   // the parent: assigned one level earlier
+                    const long long j = find_label(m, v, __ldcg(m.labels + pv));
+                    if (j >= 0 && __ldcg(m.H + j) <= __ldcg(m.hminp1 + v)) bk = (uint32_t)(j - (long long)m.ptr[v]);
+                }
+            }
+            for (uint32_t q = 0; q < nb.deg && !S; ++q) {
                 const uint32_t w = nb_at(m, nb, q);
                 const uint32_t pw = m.pos[w];
                 if (m.labels[w] != 0 && pw != NO_NODE && pw < start + i) {  // the parent: assigned one level earlier
@@ -683,8 +746,9 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
 // label bitmask [mw] u32 | prefix popcounts [mw] u16 (padded to 4 bytes)
 __host__ __device__ __forceinline__ uint32_t tree_group_bytes(uint32_t cap, uint32_t mw) { return cap * 6u + mw * 4u + ((mw * 2u + 3u) & ~3u); }
 
-// W: weighted Potts terms (slot_weight); the unweighted instantiation is the face-graph solver
-template <int G, int MINB, bool W = false>
+// W: weighted Potts terms (slot_weight); the unweighted instantiation is the face-graph solver.  S: a spanning forest (only
+// the global-memory recursion differs: k_tree_prep<true> has classified the neighbours for the fast path)
+template <int G, int MINB, bool W = false, bool S = false>
 __global__ void __launch_bounds__(TREE_THREADS, MINB) k_tree(Mrf m)
 {
     if (__ldcg(m.state + ST_STOP)) return;
@@ -712,7 +776,7 @@ __global__ void __launch_bounds__(TREE_THREADS, MINB) k_tree(Mrf m)
         const uint32_t cnt = te.x & 0x7FFFFFFFu, start = te.z;
         if (te.x >> 31) {   // a node of degree > 3 or a label list longer than the scratch
             if (lane == 0) atomicAdd(m.state + ST_SLOW, 1u);
-            tree_solve_global<W>(m, start, cnt, lane);
+            tree_solve_global<W, S>(m, start, cnt, lane);
             continue;
         }
         NodeRec *rec = m.rec + start;
@@ -902,6 +966,29 @@ __global__ void k_stop(Mrf m, uint32_t t, uint32_t window, float ratio, uint32_t
     if (stop) m.state[ST_STOP] = t;
 }
 
+// Acceptance of spanning iteration t, after k_energy and before k_restore and k_stop: fixing the non-tree neighbours at
+// their old labels does not guarantee descent, so an iteration that raised the energy keeps the energy (and, through
+// k_restore, the labels) of the iteration before.  One thread decides; k_restore only reads the decision.
+__global__ void k_accept(Mrf m, uint32_t t)
+{
+    if (m.state[ST_STOP]) return;
+    const long long e0 = (long long)m.efix[t - 1], e1 = (long long)m.efix[t];
+    if (e1 > e0) {
+        m.efix[t] = (unsigned long long)e0;
+        m.ctl[CTL_REJECT] = 1u;
+        m.state[ST_REJECTED] += 1u;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_restore(Mrf m)
+{
+    if (__ldcg(m.state + ST_STOP) || !__ldcg(m.ctl + CTL_REJECT)) return;
+    for (uint32_t v = m.nb + blockIdx.x * blockDim.x + threadIdx.x; v < m.ne; v += gridDim.x * blockDim.x) {
+        m.labels[v] = m.snap[v];
+        m.lidx[v] = m.snap_lidx[v];
+    }
+}
+
 // label range check + unseen count (view_selection.cpp:121-132)
 __global__ void __launch_bounds__(256) k_label_check(Mrf m)
 {
@@ -1079,6 +1166,8 @@ Mrf make_mrf(b2tex_ctx *c, uint32_t iter)
     m.M = c->mrf_M.p; m.J = c->mrf_J.p; m.mstride = c->nnz;
     m.tree_cap = c->mrf_tree_cap;
     m.wgt = nullptr;
+    m.par = c->mrf_par.p;
+    m.snap = c->mrf_snap.p; m.snap_lidx = c->mrf_snap.p ? c->mrf_snap.p + c->F : nullptr;
     return m;
 }
 
@@ -1110,12 +1199,13 @@ int coop_grid(b2tex_ctx *c, K kernel, size_t smem, int *grid, int threads = 256)
     return B2TEX_OK;
 }
 
+template <bool S = false>
 int launch_forest(b2tex_ctx *c, Mrf &m, int build_trees)
 {
     cudaStream_t s = c->stream;
     int grid = 0;
     // few fat blocks: the cost of grid.sync() grows with the number of blocks
-    B2_TRY(coop_grid(c, k_forest, 0, &grid, FOREST_THREADS));
+    B2_TRY(coop_grid(c, k_forest<S>, 0, &grid, FOREST_THREADS));
     if (grid > c->num_sms) grid = c->num_sms;  // one fat block per SM: cheapest grid.sync()
     if (const char *e = getenv("B2TEX_FOREST_BLOCKS_PER_SM")) grid = c->num_sms * std::max(1, atoi(e));
     uint32_t n = m.ne - m.nb;
@@ -1124,36 +1214,36 @@ int launch_forest(b2tex_ctx *c, Mrf &m, int build_trees)
     B2_CUDA(cudaMemsetAsync(m.ctl, 0, CTL_WORDS * sizeof(uint32_t), s));
     void *args[] = {&m, &build_trees};
     count_launch();
-    B2_CUDA(cudaLaunchCooperativeKernel((void *)k_forest, dim3(grid), dim3(FOREST_THREADS), args, 0, s));
+    B2_CUDA(cudaLaunchCooperativeKernel((void *)k_forest<S>, dim3(grid), dim3(FOREST_THREADS), args, 0, s));
     return B2TEX_OK;
 }
 
-template <int G, int MINB, bool W>
+template <int G, int MINB, bool W, bool S>
 int launch_tree_variant(b2tex_ctx *c, Mrf &m)
 {
     static bool attr_set = false;   // opt in to > 48 KB of dynamic shared memory (per function, once)
     if (!attr_set) {
-        B2_CUDA(cudaFuncSetAttribute(k_tree<G, MINB, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        B2_CUDA(cudaFuncSetAttribute(k_tree<G, MINB, W, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         attr_set = true;
     }
     int per_sm = 0;
-    B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_tree<G, MINB, W>, TREE_THREADS, m.tree_smem));
+    B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_tree<G, MINB, W, S>, TREE_THREADS, m.tree_smem));
     if (per_sm < 1) { set_error("k_tree cannot be resident with %u bytes of shared memory", m.tree_smem); return B2TEX_ERR_CUDA; }
     const int grid = c->num_sms * per_sm;
-    B2_LAUNCH k_tree<G, MINB, W><<<grid, TREE_THREADS, m.tree_smem, c->stream>>>(m);
+    B2_LAUNCH k_tree<G, MINB, W, S><<<grid, TREE_THREADS, m.tree_smem, c->stream>>>(m);
     B2_KERNEL_CHECK();
     return B2TEX_OK;
 }
 
-template <int G, bool W = false>
+template <int G, bool W = false, bool S = false>
 int launch_tree(b2tex_ctx *c, Mrf &m)
 {
     const uint32_t n = m.ne - m.nb;
-    B2_LAUNCH k_tree_prep<<<(n + 255) / 256, 256, 0, c->stream>>>(m);   // at most n forest nodes; the kernel reads the count
+    B2_LAUNCH k_tree_prep<S><<<(n + 255) / 256, 256, 0, c->stream>>>(m);   // at most n forest nodes; the kernel reads the count
     // 2 CTAs of 512 threads per SM (64 registers) or 3 (40 registers, a few spills): the kernel lives on resident warps, but
     // on an H100 SXM (700 W) the spill-free variant is faster (C3: k_tree 28.7 against 44.6 ms per pass)
     static const int minb = getenv("B2TEX_TREE_BLOCKS") ? atoi(getenv("B2TEX_TREE_BLOCKS")) : 2;
-    return minb == 3 ? launch_tree_variant<G, 3, W>(c, m) : launch_tree_variant<G, 2, W>(c, m);
+    return minb == 3 ? launch_tree_variant<G, 3, W, S>(c, m) : launch_tree_variant<G, 2, W, S>(c, m);
 }
 
 // peers of this context, or nranks == 1
@@ -1187,8 +1277,9 @@ int launch_energy(b2tex_ctx *c, Mrf &m, uint32_t t)
 }
 
 // label halo -> barrier -> partial energies -> barrier + all-reduce + stop rule (multi-GPU), or energy + stop rule.
-// t_ref: the iteration the stop rule's window restarts from (a phase of multilevel view selection, single GPU only)
-int enqueue_exchange_and_energy(b2tex_ctx *c, Mrf &m, uint32_t t, bool stop_rule, uint32_t t_ref = 0)
+// t_ref: the iteration the stop rule's window restarts from (a phase of multilevel or spanning-tree view selection, single
+// GPU only).  accept: a spanning iteration, undone if it raised the energy (single GPU only).
+int enqueue_exchange_and_energy(b2tex_ctx *c, Mrf &m, uint32_t t, bool stop_rule, uint32_t t_ref = 0, bool accept = false)
 {
     cudaStream_t s = c->stream;
     const b2tex_mrf_params &p = c->mrf_params;
@@ -1197,6 +1288,11 @@ int enqueue_exchange_and_energy(b2tex_ctx *c, Mrf &m, uint32_t t, bool stop_rule
         {
             ScopedTimer te(c, "mrf.k_energy", 12.0 * (double)(m.ne - m.nb));
             B2_TRY(launch_energy(c, m, t));
+        }
+        if (accept) {
+            ScopedTimer ta(c, "mrf.accept");
+            B2_LAUNCH k_accept<<<1, 1, 0, s>>>(m, t);
+            B2_LAUNCH k_restore<<<std::max(1, c->num_sms * 8), 256, 0, s>>>(m);
         }
         if (stop_rule) {   // k_stop on the phase's own iteration numbers: ST_STOP / ST_DONE are relative to t_ref
             Mrf ms = m;
@@ -1241,6 +1337,25 @@ int enqueue_iteration(b2tex_ctx *c, Mrf &m, bool stop_rule, uint32_t t_ref = 0)
         }
     }
     return enqueue_exchange_and_energy(c, m, m.iter, stop_rule, t_ref);
+}
+
+// one iteration on the spanning forest (single GPU, whole mesh), accepted or undone, and the stop rule (window from t_ref)
+int enqueue_spanning_iteration(b2tex_ctx *c, Mrf &m, uint32_t t_ref)
+{
+    {
+        ScopedTimer tf(c, "mrf.k_forest_spanning");
+        B2_TRY(launch_forest<true>(c, m, 1));
+    }
+    {
+        ScopedTimer tu(c, "mrf.k_tree_spanning");
+        switch (c->mrf_group) {
+            case 4: B2_TRY((launch_tree<4, false, true>(c, m))); break;
+            case 8: B2_TRY((launch_tree<8, false, true>(c, m))); break;
+            case 16: B2_TRY((launch_tree<16, false, true>(c, m))); break;
+            default: B2_TRY((launch_tree<32, false, true>(c, m))); break;
+        }
+    }
+    return enqueue_exchange_and_energy(c, m, m.iter, true, t_ref, true);
 }
 
 // one iteration of the BCD on the contracted MRF (weighted Potts terms), the projection onto the faces, and the fine
@@ -1317,6 +1432,10 @@ int alloc_mrf(b2tex_ctx *c, const b2tex_mrf_params *p)
     B2_TRY(c->mrf_energy.zero(c->stream));
     static const bool forest_timing = getenv("B2TEX_FOREST_TIMING") != nullptr;
     if (forest_timing) { B2_TRY(c->mrf_dbg.alloc(16)); B2_TRY(c->mrf_dbg.zero(c->stream)); }
+    if (p->use_spanning_tree) {   // parents, and the labels and label positions at the start of an iteration
+        B2_TRY(c->mrf_par.alloc(F));
+        B2_TRY(c->mrf_snap.alloc(2 * F));
+    }
     B2_TRY(c->mrf_adj4.alloc(F));
     if (F) B2_LAUNCH k_build_adj4<<<(unsigned)((F + 255) / 256), 256, 0, c->stream>>>((uint32_t)F, c->adj_ptr.p, c->adj_idx.p, c->mrf_adj4.p);
     if (!(c->valid & LABELS) || c->labels.n != F) { B2_TRY(c->labels.alloc(F)); B2_TRY(c->labels.zero(c->stream)); }
@@ -1411,9 +1530,9 @@ int mrf_prepare(b2tex_ctx *c, const b2tex_mrf_params *p)
     // ... and every kernel of the run is loaded now: with lazy module loading the FIRST launch of a kernel synchronises
     // the context, which would also wait for a peer rank's spinning barrier kernel
     cudaFuncAttributes fa;
-    const void *fns[] = {(const void *)k_forest, (const void *)k_energy, (const void *)k_stop, (const void *)k_label_check,
+    const void *fns[] = {(const void *)k_forest<false>, (const void *)k_energy, (const void *)k_stop, (const void *)k_label_check,
                          (const void *)k_build_adj4, (const void *)k_halo_build, (const void *)k_halo_push, (const void *)k_range_push,
-                         (const void *)k_mg_sync, (const void *)k_tree_prep, (const void *)k_max_labels, (const void *)k_tree<4, 3>, (const void *)k_tree<8, 3>, (const void *)k_tree<16, 3>,
+                         (const void *)k_mg_sync, (const void *)k_tree_prep<false>, (const void *)k_max_labels, (const void *)k_tree<4, 3>, (const void *)k_tree<8, 3>, (const void *)k_tree<16, 3>,
                          (const void *)k_tree<32, 3>, (const void *)k_tree<4, 2>, (const void *)k_tree<8, 2>, (const void *)k_tree<16, 2>,
                          (const void *)k_tree<32, 2>, (const void *)k_init_labels<4>, (const void *)k_init_labels<8>,
                          (const void *)k_init_labels<16>, (const void *)k_init_labels<32>};
@@ -1440,7 +1559,8 @@ int mrf_iterate(b2tex_ctx *c, uint32_t t, int64_t *efix)
 // queues iterations ahead of the device; the stop rule is evaluated on the device and turns the launches that are already
 // queued behind it into no-ops.  With peers attached (mrf_mg_export / mrf_mg_import) every rank runs this same loop; the
 // ranks meet inside the kernels.
-int run_phase(b2tex_ctx *c, uint32_t t_begin, uint32_t t_ref, bool coarse)
+enum class Phase { fine, coarse, spanning };
+int run_phase(b2tex_ctx *c, uint32_t t_begin, uint32_t t_ref, Phase phase)
 {
     cudaStream_t s = c->stream;
     const uint32_t max_it = c->mrf_params.max_iterations;
@@ -1451,7 +1571,8 @@ int run_phase(b2tex_ctx *c, uint32_t t_begin, uint32_t t_ref, bool coarse)
     int rc = B2TEX_OK;
     for (uint32_t t = t_begin; t <= max_it; ++t) {
         Mrf m = make_mrf(c, t);
-        rc = coarse ? enqueue_coarse_iteration(c, t, t_ref) : enqueue_iteration(c, m, true, t_ref);
+        rc = phase == Phase::coarse ? enqueue_coarse_iteration(c, t, t_ref)
+             : phase == Phase::spanning ? enqueue_spanning_iteration(c, m, t_ref) : enqueue_iteration(c, m, true, t_ref);
         if (rc != B2TEX_OK) break;
         const int slot = (int)(t % (LAG + 1));
         if (cudaMemcpyAsync((void *)&hf[slot], m.state + ST_STOP, 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
@@ -1485,15 +1606,16 @@ int phase_end(b2tex_ctx *c, uint32_t t_ref, uint32_t *t_end)
     return B2TEX_OK;
 }
 
-// The multilevel schedule of oracle/mrf_multilevel.c, after the first fine phase: contract the labeling, run the BCD on
-// the contracted MRF from the current labels (every iteration projected, the trace and the stop rule on fine energies,
-// window restarted), and go back to a fine phase while the coarse phase strictly lowered the energy.
+// The multilevel schedule of oracle/mrf_multilevel.c, after the first fine phase (which started after *t_ref): contract
+// the labeling, run the BCD on the contracted MRF from the current labels (every iteration projected, the trace and the
+// stop rule on fine energies, window restarted), and go back to a fine phase while the coarse phase strictly lowered the
+// energy.
 int run_multilevel(b2tex_ctx *c, b2tex_mrf_info *info, uint32_t *t_ref)
 {
     const uint32_t max_it = c->mrf_params.max_iterations;
     const Mrf m = make_mrf(c, 0);
     uint32_t t = 0;
-    B2_TRY(phase_end(c, 0, &t));
+    B2_TRY(phase_end(c, *t_ref, &t));
     while (t < max_it) {
         int64_t before = 0, after = 0;
         B2_TRY(read_energy(c, m, t, &before));
@@ -1506,7 +1628,7 @@ int run_multilevel(b2tex_ctx *c, b2tex_mrf_info *info, uint32_t *t_ref)
         }
         info->coarse_nodes = n;
         B2_CUDA(cudaMemsetAsync(m.state + ST_STOP, 0, sizeof(uint32_t), c->stream));
-        B2_TRY(run_phase(c, t + 1, t, true));
+        B2_TRY(run_phase(c, t + 1, t, Phase::coarse));
         *t_ref = t;
         uint32_t t2 = 0;
         B2_TRY(phase_end(c, t, &t2));
@@ -1515,21 +1637,26 @@ int run_multilevel(b2tex_ctx *c, b2tex_mrf_info *info, uint32_t *t_ref)
         info->multilevel_passes++;
         if (t2 >= max_it) break;
         B2_CUDA(cudaMemsetAsync(m.state + ST_STOP, 0, sizeof(uint32_t), c->stream));
-        B2_TRY(run_phase(c, t2 + 1, t2, false));
+        B2_TRY(run_phase(c, t2 + 1, t2, Phase::fine));
         *t_ref = t2;
         B2_TRY(phase_end(c, t2, &t));
     }
     return B2TEX_OK;
 }
 
-// The whole run: init, the iterations (run_phase), and with use_multilevel the multilevel schedule (run_multilevel).
+// The whole run: init, with use_spanning_tree the spanning phase, the iterations on induced forests (run_phase), and with
+// use_multilevel the multilevel schedule (run_multilevel).
 int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, double *trace)
 {
     info->multilevel_passes = 0;
     info->coarse_nodes = 0;
-    if (p->use_multilevel && ((p->num_parts ? p->num_parts : 1) > 1 || mg_active(c) || c->face_begin != 0 || c->face_end != c->F)) {
-        set_error("multilevel view selection: one GPU and the whole mesh only (num_parts %u, %s, face range %u..%u of %u)",
-                  p->num_parts, mg_active(c) ? "peers attached" : "no peers", c->face_begin, c->face_end, c->F);
+    info->spanning_tree_iterations = 0;
+    info->spanning_tree_rejected = 0;
+    if ((p->use_multilevel || p->use_spanning_tree) &&
+        ((p->num_parts ? p->num_parts : 1) > 1 || mg_active(c) || c->face_begin != 0 || c->face_end != c->F)) {
+        set_error("%s view selection: one GPU and the whole mesh only (num_parts %u, %s, face range %u..%u of %u)",
+                  p->use_spanning_tree ? "spanning-tree" : "multilevel", p->num_parts,
+                  mg_active(c) ? "peers attached" : "no peers", c->face_begin, c->face_end, c->F);
         return B2TEX_ERR_UNSUPPORTED;
     }
     int64_t e0 = 0;
@@ -1546,8 +1673,20 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
         return B2TEX_OK;
     }
     invalidate(c, LABELS);   // until the iterations below have finished without error
-    B2_TRY(run_phase(c, 1, 0, false));
     uint32_t t_ref = 0;   // the stop rule's reference iteration of the last phase: ST_STOP / ST_DONE count from it
+    if (p->use_spanning_tree) {
+        B2_TRY(run_phase(c, 1, 0, Phase::spanning));
+        uint32_t t_sp = 0;
+        B2_TRY(phase_end(c, 0, &t_sp));
+        info->spanning_tree_iterations = t_sp;
+        if (t_sp < max_it) {   // the acyclic phase from those labels, window restarted
+            B2_CUDA(cudaMemsetAsync(c->mrf_state.p + ST_STOP, 0, sizeof(uint32_t), s));
+            B2_TRY(run_phase(c, t_sp + 1, t_sp, Phase::fine));
+            t_ref = t_sp;
+        }
+    } else {
+        B2_TRY(run_phase(c, 1, 0, Phase::fine));
+    }
     if (p->use_multilevel) B2_TRY(run_multilevel(c, info, &t_ref));
     Mrf m = make_mrf(c, 0);
     if (mg) {   // one all-gather of the final labels by peer stores: seam leveling assembles its system on every rank
@@ -1577,6 +1716,7 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
     info->energy_initial = (double)(int64_t)efix[0] / 4294967296.0;
     info->energy_final = (double)(int64_t)efix[t_end] / 4294967296.0;
     info->unseen = st[ST_UNSEEN];
+    info->spanning_tree_rejected = st[ST_REJECTED];
     if (trace) for (uint32_t t = 0; t <= t_end; ++t) trace[t] = (double)(int64_t)efix[t] / 4294967296.0;
     // roofline accounting of k_tree: SURVEY 8d's sweep formula restricted to the nodes the launches processed
     unsigned long long fn, fz;
