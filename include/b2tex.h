@@ -94,6 +94,14 @@ typedef struct {
     uint32_t coarse_nodes;        /* use_multilevel: nodes of the last contraction */
     uint32_t spanning_tree_iterations;   /* use_spanning_tree: iterations of the spanning phase (numbered 1 ..) */
     uint32_t spanning_tree_rejected;     /* use_spanning_tree: of those, the ones that were undone */
+    /* how the tree solver (k_tree) ran, fixed per run from the input */
+    uint32_t tree_group;         /* lanes per tree node: 4, 8, 16 or 32, from the candidates per face */
+    uint32_t tree_cap;           /* longest label list the shared-memory scratch holds; trees with a longer list are
+                                    solved through global memory */
+    uint32_t label_mask_words;   /* 32-bit words of the per-node label bitmask (0: more than 2047 views, labels found
+                                    by bisection of the sorted list) */
+    uint32_t global_trees;       /* trees solved through global memory (a node of degree > 3 or a label list longer
+                                    than tree_cap), summed over all iterations and phases */
 } b2tex_mrf_info;
 
 typedef struct {

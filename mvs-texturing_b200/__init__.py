@@ -68,7 +68,9 @@ class B2MrfInfo(C.Structure):
     _fields_ = [("iterations", C.c_uint32), ("energy_initial", C.c_double),
                 ("energy_final", C.c_double), ("unseen", C.c_uint64), ("sweep_bytes", C.c_uint64),
                 ("multilevel_passes", C.c_uint32), ("coarse_nodes", C.c_uint32),
-                ("spanning_tree_iterations", C.c_uint32), ("spanning_tree_rejected", C.c_uint32)]
+                ("spanning_tree_iterations", C.c_uint32), ("spanning_tree_rejected", C.c_uint32),
+                ("tree_group", C.c_uint32), ("tree_cap", C.c_uint32), ("label_mask_words", C.c_uint32),
+                ("global_trees", C.c_uint32)]
 
 
 class B2PatchInfo(C.Structure):

@@ -537,6 +537,7 @@ __global__ void __launch_bounds__(FOREST_THREADS, 1) k_forest(Mrf m, int build_t
 // through the global tables H / hminp1 / amin (tree_solve_global).
 constexpr int TREE_THREADS = 512;
 constexpr int TREE_WARPS = TREE_THREADS / 32;
+constexpr uint32_t TREE_SMEM_MAX = 200u * 1024u;   // dynamic shared memory every k_tree instance opts in to (bytes)
 constexpr uint32_t NBR_SKIP = 0u, NBR_CHILD = 1u << 30, NBR_FIXED = 2u << 30, NBR_PARENT = 3u << 30;
 constexpr uint32_t NBR_KIND = 3u << 30, NBR_ARG = ~NBR_KIND;
 
@@ -1223,7 +1224,7 @@ int launch_tree_variant(b2tex_ctx *c, Mrf &m)
 {
     static bool attr_set = false;   // opt in to > 48 KB of dynamic shared memory (per function, once)
     if (!attr_set) {
-        B2_CUDA(cudaFuncSetAttribute(k_tree<G, MINB, W, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        B2_CUDA(cudaFuncSetAttribute(k_tree<G, MINB, W, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TREE_SMEM_MAX));
         attr_set = true;
     }
     int per_sm = 0;
@@ -1455,7 +1456,8 @@ int alloc_mrf(b2tex_ctx *c, const b2tex_mrf_params *p)
     static const bool no_masks = getenv("B2TEX_NO_MASKS") != nullptr;
     c->mrf_mask_words = (c->K == 0 || words > (uint32_t)MAX_MASK_WORDS || no_masks) ? 0 : words;
     // shared-memory scratch of k_tree: one h row + label list (6 bytes per label) per lane group; the longest label
-    // list decides (longer ones -- only if a face sees more than 1024 views -- go through the global tables)
+    // list decides, up to 1024 labels and as long as the scratch of all lane groups fits TREE_SMEM_MAX (trees with a
+    // longer list go through the global tables)
     uint32_t maxn = 0;
     if (nodes) {
         B2_TRY(c->s_limits.alloc(1));
@@ -1468,9 +1470,10 @@ int alloc_mrf(b2tex_ctx *c, const b2tex_mrf_params *p)
     }
     uint32_t cap = std::min(1024u, std::max(16u, (maxn + 15u) & ~15u));
     if (const char *e = getenv("B2TEX_TREE_CAP")) cap = (uint32_t)std::max(16, std::min(1024, atoi(e) & ~15));
+    const uint32_t groups = (uint32_t)TREE_WARPS * (32u / (uint32_t)c->mrf_group);
+    while (cap > 16u && groups * tree_group_bytes(cap, c->mrf_mask_words) > TREE_SMEM_MAX) cap -= 16u;
     c->mrf_tree_cap = cap;
-    uint32_t smem = (uint32_t)TREE_WARPS * (32u / (uint32_t)c->mrf_group) * tree_group_bytes(cap, c->mrf_mask_words);
-    c->mrf_tree_smem = smem;
+    c->mrf_tree_smem = groups * tree_group_bytes(cap, c->mrf_mask_words);
     return B2TEX_OK;
 }
 
@@ -1661,6 +1664,10 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
     }
     int64_t e0 = 0;
     B2_TRY(mrf_init(c, p, &e0));
+    info->tree_group = (uint32_t)c->mrf_group;
+    info->tree_cap = c->mrf_tree_cap;
+    info->label_mask_words = c->mrf_mask_words;
+    info->global_trees = 0;
     cudaStream_t s = c->stream;
     const uint32_t max_it = p->max_iterations, window = p->window ? p->window : 1u;
     const bool mg = mg_active(c);
@@ -1717,6 +1724,7 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
     info->energy_final = (double)(int64_t)efix[t_end] / 4294967296.0;
     info->unseen = st[ST_UNSEEN];
     info->spanning_tree_rejected = st[ST_REJECTED];
+    info->global_trees = st[ST_SLOW];
     if (trace) for (uint32_t t = 0; t <= t_end; ++t) trace[t] = (double)(int64_t)efix[t] / 4294967296.0;
     // roofline accounting of k_tree: SURVEY 8d's sweep formula restricted to the nodes the launches processed
     unsigned long long fn, fz;
