@@ -82,6 +82,13 @@ typedef struct {
                                      phase follows with the window restarted, then the multilevel schedule if
                                      use_multilevel.  One GPU, whole mesh, num_parts 1 only (else B2TEX_ERR_UNSUPPORTED).
                                      Default 0. */
+    uint32_t spanning_tree_multilevel_after_n_iterations;   /* mapMAP_control's field of that name (n): with n > 0,
+                                     a multilevel step (contract the labeling, one spanning-tree iteration on the contracted
+                                     MRF with weighted Potts terms, undone if it raises the energy) follows every n-th
+                                     iteration of the spanning phase, unless the stop rule has fired or max_iterations is
+                                     reached.  The induced-forest phase follows and is the last one: the post-acyclic
+                                     multilevel schedule does not run.  n > 0 needs use_spanning_tree = 1 and
+                                     use_multilevel = 1 (else B2TEX_ERR_ARG).  Default 0. */
 } b2tex_mrf_params;
 
 typedef struct {
@@ -102,6 +109,9 @@ typedef struct {
                                     by bisection of the sorted list) */
     uint32_t global_trees;       /* trees solved through global memory (a node of degree > 3 or a label list longer
                                     than tree_cap), summed over all iterations and phases */
+    uint32_t multilevel_steps;            /* spanning_tree_multilevel_after_n_iterations > 0: multilevel steps of the
+                                             spanning phase (counted in spanning_tree_iterations, which numbers both) */
+    uint32_t multilevel_steps_rejected;   /* of those, the ones that were undone (not in spanning_tree_rejected) */
 } b2tex_mrf_info;
 
 typedef struct {
@@ -168,6 +178,9 @@ uint64_t b2tex_launch_count(void);                /* kernels of this library lau
 int b2tex_profile(b2tex_ctx *ctx, int enable);
 int b2tex_profile_report(b2tex_ctx *ctx, char *buf, uint64_t cap);
 void b2tex_default_mrf_params(b2tex_mrf_params *p);
+/* the defaults with mapMAP's control as texrecon sets it (view_selection.cpp:103-115): use_spanning_tree = 1,
+ * use_multilevel = 1, spanning_tree_multilevel_after_n_iterations = 5 */
+void b2tex_texrecon_mrf_params(b2tex_mrf_params *p);
 
 /* ---- resident API: upload once, run stages on the device, download results ----
  *

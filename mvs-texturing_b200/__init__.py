@@ -23,7 +23,7 @@ LIB_PATH = os.path.join(_HERE, "libb2tex.so")
 EXPORTS = [
     "b2tex_create", "b2tex_destroy", "b2tex_last_error", "b2tex_free", "b2tex_device_synchronize",
     "b2tex_stream", "b2tex_launch_count", "b2tex_profile", "b2tex_profile_report",
-    "b2tex_default_mrf_params", "b2tex_set_mesh", "b2tex_set_views", "b2tex_set_adjacency",
+    "b2tex_default_mrf_params", "b2tex_texrecon_mrf_params", "b2tex_set_mesh", "b2tex_set_views", "b2tex_set_adjacency",
     "b2tex_set_vertex_rings", "b2tex_set_data_costs", "b2tex_set_labels", "b2tex_set_face_range", "b2tex_undistort_views",
     "b2tex_data_costs_run", "b2tex_data_costs_qualities", "b2tex_data_costs_histogram",
     "b2tex_data_costs_normalize", "b2tex_data_costs_download", "b2tex_view_selection_run", "b2tex_view_selection_prepare",
@@ -61,7 +61,7 @@ class B2MrfParams(C.Structure):
     _fields_ = [("max_iterations", C.c_uint32), ("rounds", C.c_uint32), ("root_div", C.c_uint32),
                 ("seed", C.c_uint32), ("window", C.c_uint32), ("ratio", C.c_float),
                 ("num_parts", C.c_uint32), ("num_views", C.c_uint32), ("use_multilevel", C.c_uint32),
-                ("use_spanning_tree", C.c_uint32)]
+                ("use_spanning_tree", C.c_uint32), ("spanning_tree_multilevel_after_n_iterations", C.c_uint32)]
 
 
 class B2MrfInfo(C.Structure):
@@ -70,7 +70,8 @@ class B2MrfInfo(C.Structure):
                 ("multilevel_passes", C.c_uint32), ("coarse_nodes", C.c_uint32),
                 ("spanning_tree_iterations", C.c_uint32), ("spanning_tree_rejected", C.c_uint32),
                 ("tree_group", C.c_uint32), ("tree_cap", C.c_uint32), ("label_mask_words", C.c_uint32),
-                ("global_trees", C.c_uint32)]
+                ("global_trees", C.c_uint32), ("multilevel_steps", C.c_uint32),
+                ("multilevel_steps_rejected", C.c_uint32)]
 
 
 class B2PatchInfo(C.Structure):
@@ -155,6 +156,16 @@ def make_views(pos, viewdir, proj, w2c, width, height, images):
 def mrf_params(**kw) -> B2MrfParams:
     p = B2MrfParams()
     lib().b2tex_default_mrf_params(C.byref(p))
+    for k, v in kw.items():
+        setattr(p, k, v)
+    return p
+
+
+def texrecon_mrf_params(**kw) -> B2MrfParams:
+    """mrf_params with mapMAP's control as texrecon sets it (b2tex_texrecon_mrf_params): use_spanning_tree = 1,
+    use_multilevel = 1, spanning_tree_multilevel_after_n_iterations = 5; `kw` on top."""
+    p = B2MrfParams()
+    lib().b2tex_texrecon_mrf_params(C.byref(p))
     for k, v in kw.items():
         setattr(p, k, v)
     return p

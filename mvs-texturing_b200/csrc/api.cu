@@ -40,6 +40,15 @@ void b2tex_default_mrf_params(b2tex_mrf_params *p)
     p->num_views = 0;
     p->use_multilevel = 0;
     p->use_spanning_tree = 0;
+    p->spanning_tree_multilevel_after_n_iterations = 0;
+}
+
+void b2tex_texrecon_mrf_params(b2tex_mrf_params *p)
+{
+    b2tex_default_mrf_params(p);
+    p->use_spanning_tree = 1;
+    p->use_multilevel = 1;
+    p->spanning_tree_multilevel_after_n_iterations = 5;   // view_selection.cpp:103-115
 }
 
 int b2tex_create(int device, b2tex_ctx **out)

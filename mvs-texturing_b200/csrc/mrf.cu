@@ -29,6 +29,10 @@
 // spanning forest from the same roots and records every node's parent in `par`; k_tree_prep<true> classifies neighbours by
 // `par` (every non-tree neighbour is fixed at its label from the start of the iteration), and k_accept / k_restore undo an
 // iteration that raised the energy.
+// spanning_tree_multilevel_after_n_iterations = n (oracle/mrf_mapmap.c, texrecon's mapMAP control): inside the spanning
+// phase, after every n spanning iterations, one multilevel step -- the contraction, ONE spanning iteration on the contracted
+// MRF (k_forest<true>, k_tree_prep<true>, k_tree<G, MINB, true, true>), the projection, and k_accept on the fine energy
+// (enqueue_multilevel_step).  The acyclic phase follows and stays the last one.
 #include <cooperative_groups.h>
 #include <stdlib.h>
 #include <string.h>
@@ -105,6 +109,7 @@ constexpr int CTL_CURSOR = MAX_LEVELS + 9;       // forest nodes laid out so far
 constexpr int CTL_CLAIM = MAX_LEVELS + 10;       // k_tree: next unclaimed tree
 constexpr int CTL_REJECT = MAX_LEVELS + 11;      // spanning iteration: k_accept rejected it, k_restore brings the labels back
 constexpr int CTL_MAXPRIO = MAX_LEVELS + 12;     // 64-bit, 8-byte aligned
+constexpr int CTL_KEEP = MAX_LEVELS + 14;        // multilevel step: nonzero unless it was rejected (skips the re-projection)
 constexpr int CTL_WORDS = MAX_LEVELS + 32;
 // run state (uint32 words)
 constexpr int ST_STOP = 0;      // 0 while running, else the iteration the stop rule fired in
@@ -115,7 +120,9 @@ constexpr int ST_FNODES = 4;    // 64-bit: forest nodes summed over the iteratio
 constexpr int ST_FNNZ = 6;      // 64-bit: labels of forest nodes summed over the iterations
 constexpr int ST_SLOW = 8;      // trees that went through global memory
 constexpr int ST_ERR = 9;       // cross-GPU barrier timeouts (a peer did not arrive)
-constexpr int ST_REJECTED = 10; // spanning iterations that raised the energy and were undone
+constexpr int ST_REJECTED = 10; // spanning iterations and multilevel steps that raised the energy and were undone
+constexpr int ST_STEPS = 11;    // multilevel steps of the spanning phase
+constexpr int ST_STEP_REJ = 12; // of those, the ones that were undone
 constexpr int ST_WORDS = 16;
 
 __device__ __forceinline__ bool same_part(const Mrf &m, uint32_t a, uint32_t b)
@@ -644,7 +651,8 @@ __device__ __forceinline__ float slot_weight(const Mrf &m, uint32_t v, uint32_t 
 
 // the same recursion through global memory: any degree, any size (one node at a time, 32 lanes over its labels).
 // S: a spanning forest, classified by m.par as k_tree_prep<true> does; fixed labels come from the snapshot, because the
-// top-down passes of other warps write m.labels meanwhile and a spanning tree has edges to other trees.
+// top-down passes of other warps write m.labels meanwhile and a spanning tree has edges to other trees.  W and S together:
+// the spanning forest of a contracted MRF, the weight of the edge to the parent is that of the slot holding par[v].
 template <bool W, bool S = false>
 __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, uint32_t lane)
 {
@@ -656,7 +664,11 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
             const uint64_t p0 = m.ptr[v], p1 = m.ptr[v + 1];
             const Nb nb = load_nb(m, v);
             float wpar = 1.0f;   // weight of the edge to the parent
-            if constexpr (W) {
+            if constexpr (W && S) {
+                const uint32_t pv = m.par[v];
+                for (uint32_t q = 0; q < nb.deg; ++q)
+                    if (nb_at(m, nb, q) == pv) wpar = slot_weight<W>(m, v, q);
+            } else if constexpr (W) {
                 for (uint32_t q = 0; q < nb.deg; ++q) {
                     const uint32_t w = nb_at(m, nb, q);
                     const uint32_t pw = m.pos[w];
@@ -680,7 +692,7 @@ __device__ void tree_solve_global(const Mrf &m, uint32_t start, uint32_t cnt, ui
                             if (j >= 0) { const float hw = __ldcg(m.H + j); if (hw < msg) msg = hw; }
                             h = h + msg;
                         } else if (w != par_v) {
-                            h = h + (lab != x ? 1.0f : 0.0f);
+                            h = h + (lab != x ? slot_weight<W>(m, v, q) : 0.0f);
                         }
                         continue;
                     }
@@ -990,6 +1002,17 @@ __global__ void __launch_bounds__(256) k_restore(Mrf m)
     }
 }
 
+// After k_accept and k_restore of a multilevel step: counts the step and its rejection, and sets CTL_KEEP unless the step
+// was rejected, so that only a rejected step projects the restored coarse labels onto the faces again
+__global__ void k_step_count(Mrf m)
+{
+    const bool stopped = m.state[ST_STOP] != 0u, rejected = m.ctl[CTL_REJECT] != 0u;
+    m.ctl[CTL_KEEP] = stopped || !rejected ? 1u : 0u;
+    if (stopped) return;
+    m.state[ST_STEPS] += 1u;
+    if (rejected) m.state[ST_STEP_REJ] += 1u;
+}
+
 // label range check + unseen count (view_selection.cpp:121-132)
 __global__ void __launch_bounds__(256) k_label_check(Mrf m)
 {
@@ -1277,6 +1300,15 @@ int launch_energy(b2tex_ctx *c, Mrf &m, uint32_t t)
     return B2TEX_OK;
 }
 
+// k_stop on the phase's own iteration numbers (single GPU): ST_STOP / ST_DONE are relative to t_ref
+void enqueue_stop(b2tex_ctx *c, const Mrf &m, uint32_t t, uint32_t t_ref)
+{
+    const b2tex_mrf_params &p = c->mrf_params;
+    Mrf ms = m;
+    ms.efix = m.efix + t_ref;
+    B2_LAUNCH k_stop<<<1, 1, 0, c->stream>>>(ms, t - t_ref, p.window ? p.window : 1u, p.ratio, p.max_iterations - t_ref);
+}
+
 // label halo -> barrier -> partial energies -> barrier + all-reduce + stop rule (multi-GPU), or energy + stop rule.
 // t_ref: the iteration the stop rule's window restarts from (a phase of multilevel or spanning-tree view selection, single
 // GPU only).  accept: a spanning iteration, undone if it raised the energy (single GPU only).
@@ -1295,11 +1327,7 @@ int enqueue_exchange_and_energy(b2tex_ctx *c, Mrf &m, uint32_t t, bool stop_rule
             B2_LAUNCH k_accept<<<1, 1, 0, s>>>(m, t);
             B2_LAUNCH k_restore<<<std::max(1, c->num_sms * 8), 256, 0, s>>>(m);
         }
-        if (stop_rule) {   // k_stop on the phase's own iteration numbers: ST_STOP / ST_DONE are relative to t_ref
-            Mrf ms = m;
-            ms.efix = m.efix + t_ref;
-            B2_LAUNCH k_stop<<<1, 1, 0, s>>>(ms, t - t_ref, window, p.ratio, p.max_iterations - t_ref);
-        }
+        if (stop_rule) enqueue_stop(c, m, t, t_ref);
         B2_KERNEL_CHECK();
         return B2TEX_OK;
     }
@@ -1383,6 +1411,57 @@ int enqueue_coarse_iteration(b2tex_ctx *c, uint32_t t, uint32_t t_ref)
         B2_TRY(mrf_project(c, m.state + ST_STOP));
     }
     return enqueue_exchange_and_energy(c, m, t, true, t_ref);
+}
+
+// One multilevel step of the spanning phase (oracle/mrf_mapmap.c) as iteration t: contract the labels, one spanning-tree
+// iteration with weighted Potts terms on the contracted MRF, the projection, the fine energy and its acceptance, and the
+// stop rule (window from t_ref).  A rejected step restores the coarse labels and positions from the snapshot k_forest<true>
+// took and projects them again: every face gets the label of its region, which is the label it had when it was contracted,
+// so no snapshot of the faces is needed.  The contraction reads its sizes back; everything after it is queued.
+int enqueue_multilevel_step(b2tex_ctx *c, uint32_t t, uint32_t t_ref, uint32_t *num_nodes)
+{
+    cudaStream_t s = c->stream;
+    {
+        ScopedTimer tc(c, "mrf_ml.contract");
+        B2_TRY(mrf_contract(c, num_nodes));
+        if (*num_nodes) B2_LAUNCH k_build_adj4<<<(*num_nodes + 255) / 256, 256, 0, s>>>(*num_nodes, c->ml_cadj_ptr.p, c->ml_cadj_idx.p, c->ml_cadj4.p);
+        B2_KERNEL_CHECK();
+    }
+    if (!*num_nodes) { set_error("multilevel step: the contraction has no nodes"); return B2TEX_ERR_ARG; }
+    Mrf cm = make_coarse_mrf(c, t);
+    {
+        ScopedTimer tf(c, "mrf.k_forest_spanning");
+        B2_TRY(launch_forest<true>(c, cm, 1));
+    }
+    {
+        ScopedTimer tu(c, "mrf.k_tree_spanning_weighted");
+        switch (c->mrf_group) {
+            case 4: B2_TRY((launch_tree<4, true, true>(c, cm))); break;
+            case 8: B2_TRY((launch_tree<8, true, true>(c, cm))); break;
+            case 16: B2_TRY((launch_tree<16, true, true>(c, cm))); break;
+            default: B2_TRY((launch_tree<32, true, true>(c, cm))); break;
+        }
+    }
+    Mrf m = make_mrf(c, t);
+    {
+        ScopedTimer tp(c, "mrf_ml.project");
+        B2_TRY(mrf_project(c, m.state + ST_STOP));
+    }
+    {
+        ScopedTimer te(c, "mrf.k_energy", 12.0 * (double)(m.ne - m.nb));
+        B2_TRY(launch_energy(c, m, t));
+    }
+    {
+        ScopedTimer ta(c, "mrf.accept");
+        B2_LAUNCH k_accept<<<1, 1, 0, s>>>(m, t);
+        B2_LAUNCH k_restore<<<std::max(1, c->num_sms * 8), 256, 0, s>>>(cm);
+        B2_LAUNCH k_step_count<<<1, 1, 0, s>>>(m);
+        B2_KERNEL_CHECK();
+        B2_TRY(mrf_project(c, m.ctl + CTL_KEEP));
+    }
+    enqueue_stop(c, m, t, t_ref);
+    B2_KERNEL_CHECK();
+    return B2TEX_OK;
 }
 
 int alloc_mrf(b2tex_ctx *c, const b2tex_mrf_params *p)
@@ -1562,11 +1641,12 @@ int mrf_iterate(b2tex_ctx *c, uint32_t t, int64_t *efix)
 // queues iterations ahead of the device; the stop rule is evaluated on the device and turns the launches that are already
 // queued behind it into no-ops.  With peers attached (mrf_mg_export / mrf_mg_import) every rank runs this same loop; the
 // ranks meet inside the kernels.
+// t_last: the last iteration to queue, if before max_iterations.
 enum class Phase { fine, coarse, spanning };
-int run_phase(b2tex_ctx *c, uint32_t t_begin, uint32_t t_ref, Phase phase)
+int run_phase(b2tex_ctx *c, uint32_t t_begin, uint32_t t_ref, Phase phase, uint32_t t_last = 0xFFFFFFFFu)
 {
     cudaStream_t s = c->stream;
-    const uint32_t max_it = c->mrf_params.max_iterations;
+    const uint32_t max_it = std::min(c->mrf_params.max_iterations, t_last);
     constexpr int LAG = 3;   // iterations queued beyond the last one whose stop flag the host has seen
     cudaEvent_t ev[LAG + 1];
     for (auto &e : ev) B2_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -1647,6 +1727,26 @@ int run_multilevel(b2tex_ctx *c, b2tex_mrf_info *info, uint32_t *t_ref)
     return B2TEX_OK;
 }
 
+// The spanning phase of oracle/mrf_mapmap.c: every n spanning iterations are queued without a host round trip, and one
+// multilevel step follows them unless the stop rule has fired or the budget is spent.  Iteration numbers go on across both.
+int run_spanning_with_steps(b2tex_ctx *c, uint32_t n, b2tex_mrf_info *info)
+{
+    const uint32_t max_it = c->mrf_params.max_iterations;
+    for (uint32_t t = 1; t <= max_it;) {
+        const uint32_t last = n - 1u >= max_it - t ? max_it : t + n - 1u;
+        B2_TRY(run_phase(c, t, 0, Phase::spanning, last));   // ends with a stream synchronisation
+        uint32_t stop = 0;
+        B2_CUDA(cudaMemcpyAsync(&stop, c->mrf_state.p + ST_STOP, sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+        B2_CUDA(cudaStreamSynchronize(c->stream));
+        if (stop || last >= max_it) break;
+        uint32_t nodes = 0;
+        B2_TRY(enqueue_multilevel_step(c, last + 1u, 0, &nodes));
+        info->coarse_nodes = nodes;
+        t = last + 2u;
+    }
+    return B2TEX_OK;
+}
+
 // The whole run: init, with use_spanning_tree the spanning phase, the iterations on induced forests (run_phase), and with
 // use_multilevel the multilevel schedule (run_multilevel).
 int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, double *trace)
@@ -1655,6 +1755,14 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
     info->coarse_nodes = 0;
     info->spanning_tree_iterations = 0;
     info->spanning_tree_rejected = 0;
+    info->multilevel_steps = 0;
+    info->multilevel_steps_rejected = 0;
+    const uint32_t every = p->spanning_tree_multilevel_after_n_iterations;
+    if (every && (!p->use_spanning_tree || !p->use_multilevel)) {
+        set_error("view selection: spanning_tree_multilevel_after_n_iterations = %u needs use_spanning_tree = 1 and "
+                  "use_multilevel = 1 (%u, %u)", every, p->use_spanning_tree, p->use_multilevel);
+        return B2TEX_ERR_ARG;
+    }
     if ((p->use_multilevel || p->use_spanning_tree) &&
         ((p->num_parts ? p->num_parts : 1) > 1 || mg_active(c) || c->face_begin != 0 || c->face_end != c->F)) {
         set_error("%s view selection: one GPU and the whole mesh only (num_parts %u, %s, face range %u..%u of %u)",
@@ -1682,7 +1790,8 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
     invalidate(c, LABELS);   // until the iterations below have finished without error
     uint32_t t_ref = 0;   // the stop rule's reference iteration of the last phase: ST_STOP / ST_DONE count from it
     if (p->use_spanning_tree) {
-        B2_TRY(run_phase(c, 1, 0, Phase::spanning));
+        if (every) B2_TRY(run_spanning_with_steps(c, every, info));
+        else B2_TRY(run_phase(c, 1, 0, Phase::spanning));
         uint32_t t_sp = 0;
         B2_TRY(phase_end(c, 0, &t_sp));
         info->spanning_tree_iterations = t_sp;
@@ -1694,7 +1803,7 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
     } else {
         B2_TRY(run_phase(c, 1, 0, Phase::fine));
     }
-    if (p->use_multilevel) B2_TRY(run_multilevel(c, info, &t_ref));
+    if (p->use_multilevel && !every) B2_TRY(run_multilevel(c, info, &t_ref));   // with steps, the acyclic phase is the last
     Mrf m = make_mrf(c, 0);
     if (mg) {   // one all-gather of the final labels by peer stores: seam leveling assembles its system on every rank
         MrfPeers pr = make_peers(c);
@@ -1723,7 +1832,9 @@ int mrf_run(b2tex_ctx *c, const b2tex_mrf_params *p, b2tex_mrf_info *info, doubl
     info->energy_initial = (double)(int64_t)efix[0] / 4294967296.0;
     info->energy_final = (double)(int64_t)efix[t_end] / 4294967296.0;
     info->unseen = st[ST_UNSEEN];
-    info->spanning_tree_rejected = st[ST_REJECTED];
+    info->spanning_tree_rejected = st[ST_REJECTED] - st[ST_STEP_REJ];
+    info->multilevel_steps = st[ST_STEPS];
+    info->multilevel_steps_rejected = st[ST_STEP_REJ];
     info->global_trees = st[ST_SLOW];
     if (trace) for (uint32_t t = 0; t <= t_end; ++t) trace[t] = (double)(int64_t)efix[t] / 4294967296.0;
     // roofline accounting of k_tree: SURVEY 8d's sweep formula restricted to the nodes the launches processed
